@@ -1,4 +1,4 @@
-"""aero_b200: B200-native implementation of the AERO generator forward path.
+"""aero_b200: H100-native (sm_90a) implementation of the AERO generator forward path.
 
 Public surface (mirrors the reference's ``src.models`` names):
   * ``Aero``                 -- drop-in for ``src.models.aero.Aero``

@@ -1,4 +1,4 @@
-"""Build libaero_b200.so for sm_100a with nvcc (in-tree; the .so travels to the GPU box)."""
+"""Build libaero_b200.so for sm_90a with nvcc, in the package directory."""
 from __future__ import annotations
 
 import glob
@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libaero_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O3"]
 
 

@@ -131,7 +131,7 @@ def load(path=None):
     path = path or LIB_PATH
     if not os.path.exists(path):
         raise AeroLibraryError(
-            f"{path} not found: build it with `python -m aero_b200.build` (nvcc, sm_100a). "
+            f"{path} not found: build it with `python -m aero_b200.build` (nvcc, sm_90a). "
             "aero_b200 has no CPU / eager fallback.")
     try:
         lib = C.CDLL(path)

@@ -1,4 +1,4 @@
-// Shared helpers for libaero_b200 (sm_100a).  No torch / ATen types anywhere in csrc/.
+// Shared helpers for libaero_b200 (sm_90a).  No torch / ATen types anywhere in csrc/.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

@@ -219,7 +219,7 @@ __global__ void __launch_bounds__(256) freq_mix_small_kernel(const TA* __restric
 template <int F>
 static int freq_mix_small_go(const void* x, const float* W, const float* gate, void* out, int B, int64_t M, int flags, cudaStream_t st) {
     int blocks = (int)((M / 4 + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     dim3 grid(blocks < 1 ? 1 : blocks, B);
     const bool a16 = flags & AERO_TG_A_F16, o16 = flags & AERO_TG_OUT_F16;
     if (a16 && o16) freq_mix_small_kernel<F, __half, __half><<<grid, 256, 0, st>>>((const __half*)x, W, gate, (__half*)out, M, flags);

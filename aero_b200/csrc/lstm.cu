@@ -145,7 +145,7 @@ extern "C" int aero_lstm_rec_fwd(const void* gin_, const float* bias_pad, const 
                                  const aero_lstm_params* p, aero_stream_t stream) {
     using namespace aero;
     AERO_REQUIRE(gin_ && whh && hout && p, "aero_lstm_rec_fwd: null argument");
-    AERO_REQUIRE(!(p->flags & AERO_TG_A_F16) || p->precision == 1, "aero_lstm_rec_fwd: FP16 gate pre-activations need the tcgen05 recurrence");
+    AERO_REQUIRE(!(p->flags & AERO_TG_A_F16) || p->precision == 1, "aero_lstm_rec_fwd: FP16 gate pre-activations need the wgmma recurrence");
     const float* gin = static_cast<const float*>(gin_);
     AERO_REQUIRE(p->rows >= 1 && p->T >= 1 && p->n_win >= 1 && p->steps >= 1, "aero_lstm_rec_fwd: bad sizes");
     AERO_REQUIRE(p->in_windowed || bias_pad, "aero_lstm_rec_fwd: bias_pad required for un-windowed input");

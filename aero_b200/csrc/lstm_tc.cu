@@ -1,25 +1,26 @@
-// Persistent BiLSTM recurrence on tcgen05 (sm_100a).  See include/aero_b200.h (aero_lstm_rec_fwd,
+// Persistent BiLSTM recurrence on the Hopper tensor cores (wgmma, sm_90a).  See include/aero_b200.h (aero_lstm_rec_fwd,
 // precision = 1).
 //
 // Per step the recurrent term is the small GEMM  D[gate rows x sequences] = W_hh[gate rows x H] * h^T[H x sequences]:
 //   A = W_hh, loaded ONCE by TMA into shared memory (K-major, SWIZZLE_128B) and resident for all steps.
 //       Gate rows are re-ordered into 128-row M tiles so that a thread finds the gates it needs in its
-//       own TMEM lane (or one xor-16 shuffle away):
+//       own accumulator row (or one xor-16 shuffle away):
 //         GPT = 1 (64 < H <= 128): tile g holds gate g, lane = cell             -> 4 tiles, no exchange
 //         GPT = 2 (32 < H <=  64): tile t holds gates (2t, 2t+1); in every warp lanes 0-15 carry gate 2t
 //                                  and lanes 16-31 gate 2t+1 of the same 16 cells -> 2 tiles, one shfl.xor 16
 //   B = h of the previous step, written by the cell-update threads straight into the swizzled
 //       shared-memory operand layout, 16 sequences per CTA;
-//   operands are FP16 (kind::f16, K = 16 per UMMA): h is in (-1, 1) and W_hh is O(1), so FP16's 10-bit mantissa gives
+//   operands are FP16 (K = 16 per wgmma): h is in (-1, 1) and W_hh is O(1), so FP16's 10-bit mantissa gives
 //       the same rounding as TF32 at half the shared-memory traffic and half the instruction count; accumulation is fp32;
-//   D = (4/GPT) x 16 fp32 columns of TMEM, read back with tcgen05.ld by the same threads.
+//   D = (4/GPT) tiles of 128 rows x 16 fp32 columns: the MMA warpgroup holds them in registers (two m64n16 accumulators per
+//       tile), writes them to a padded shared-memory tile and the cell-update threads read their row back.
 // The input-projection gate pre-activations keep PyTorch's [dir][i,f,g,o][H] column order (a warp reads the contiguous
 // cells of one gate per sequence); with one CTA per SM (GPT = 1) they are requested a whole step ahead.
-// Round 2: a CTA owns SEQ = 8 or 16 sequences (the UMMA N stays 16; unused operand rows are zero).  With 8, and W_hh for
-// 64 < H <= 96 held in 32-column SWIZZLE_64B chunks (96 KB instead of 128 KB, no zero K padding: 24 UMMAs per step instead
-// of 32), two CTAs share an SM: one CTA's MMA / barrier latency overlaps the other's exp-heavy cell update, and the
-// sequences spread over all SMs instead of 96 of them.
-// One elected lane issues the MMAs back to back from step-invariant descriptors; two mbarriers ping-pong between
+// A CTA owns SEQ = 8 or 16 sequences (the wgmma N stays 16; unused operand rows are zero).  With 8, W_hh for 64 < H <= 96 is
+// held in 32-column SWIZZLE_64B chunks (96 KB instead of 128 KB, no zero K padding: 3/4 of the wgmmas per step) and the
+// sequences spread over twice as many SMs; for H <= 64 two CTAs share an SM and one CTA's MMA / barrier latency overlaps
+// the other's exp-heavy cell update.
+// Warps 0..3 are the MMA warpgroup (warp 0 also loads W_hh) and issue the wgmmas from step-invariant descriptors; two mbarriers ping-pong between
 // "h ready" and "accumulators ready".  c stays in registers for the whole sequence.  8 (GPT = 2) or 16 (GPT = 1)
 // cell-update warps; in the two-gates-per-tile layout a lane finishes only its own half of the warp's sequences.
 #include <cuda_fp16.h>
@@ -38,7 +39,8 @@ extern "C" int aero_debug_lstm_trace(long long* host) {
 
 namespace aero {
 
-constexpr int kNT = 16;          // UMMA N (operand rows of h); a CTA fills SEQ = 8 or 16 of them
+constexpr int kNT = 16;          // wgmma N (operand rows of h); a CTA fills SEQ = 8 or 16 of them
+constexpr int kLdAcc = kNT + 4;  // row stride (floats) of the staged accumulators: lane-per-row 16-byte reads hit distinct banks
 
 // tuning knob, read from the environment once: AERO_LSTM_SEQ = 8 / 16 forces the CTA size (0 / unset: chosen per launch)
 static int lstm_seq_knob() {
@@ -50,7 +52,6 @@ struct LstmTcShared {
     uint64_t w_full;
     uint64_t acc_ready;
     uint64_t h_ready;
-    uint32_t tmem_base;
 };
 
 // ex2.approx / rcp.approx: <= 2 ulp each, i.e. ~1e-7 relative on the gates (far below the operand rounding)
@@ -65,60 +66,15 @@ __device__ __forceinline__ float fast_rcp(float x) {
     return y;
 }
 
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "r"(taddr)
-        : "memory");
-}
-
-// tcgen05.mma kind::f16 with the two shared-memory descriptors given as (low word, common high word) and a compile-time
-// accumulate flag: nothing but the low-word add is left on the issuing thread's dependency chain
-template <bool ACC>
-__device__ __forceinline__ void umma_f16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %3};\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}"
-        ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "n"(ACC ? 1 : 0)
-        : "memory");
-}
-
 template <typename T> __device__ __forceinline__ T to_storage(float v);
 template <> __device__ __forceinline__ float to_storage<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half to_storage<__half>(float v) { return __float2half_rn(v); }
 
-template <int NSQ>
-__device__ __forceinline__ void tmem_ld_n(uint32_t taddr, uint32_t (&r)[NSQ]);
-template <>
-__device__ __forceinline__ void tmem_ld_n<8>(uint32_t taddr, uint32_t (&r)[8]) { tmem_ld8(taddr, r); }
-template <>
-__device__ __forceinline__ void tmem_ld_n<4>(uint32_t taddr, uint32_t (&r)[4]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-        : "r"(taddr)
-        : "memory");
-}
-
-// K-major shared-memory matrix descriptor for a swizzled operand whose rows are ROWB bytes (128: SWIZZLE_128B, layout type 2;
-// 64: SWIZZLE_64B, layout type 4); 8-row groups are ROWB * 8 bytes apart (SBO)
-template <int ROWB>
-__device__ __forceinline__ uint64_t make_desc_kmajor(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)((ROWB * 8) >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)(ROWB == 128 ? 2 : 4) << 61);
-}
-
-// GPT: gates per 128-row tile.  NEW: cell-update warps (NEW/4 per TMEM lane quarter, each owning 4*SEQ/NEW sequences).
+// GPT: gates per 128-row tile.  NEW: cell-update warps (NEW/4 per 32-row quarter of a tile, each owning 4*SEQ/NEW sequences).
 // SEQ: sequences per CTA (8 or 16).  ROWB: bytes of K per operand row of a chunk (128 = 64 fp16, SWIZZLE_128B; 64 = 32 fp16,
 // SWIZZLE_64B).  MINB: CTAs per SM the register budget is set for.
 template <int GPT, int NEW, int SEQ, int ROWB, int MINB, typename TO, typename TG>
-__global__ void __launch_bounds__(64 + 32 * NEW, MINB)
+__global__ void __launch_bounds__(128 + 32 * NEW, MINB)
 lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ gin, const float* __restrict__ bias_pad,
                TO* __restrict__ hout, const aero_lstm_params p, const int nK) {
     constexpr int NM = 4 / GPT;                          // M tiles
@@ -129,7 +85,8 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ 
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* sA = smem;                                  // [NM][nK] tiles of 128 rows x ROWB bytes
     uint8_t* sB = smem + NM * nK * kATile;               // [nK] tiles of 16 rows x ROWB bytes
-    LstmTcShared* sh = reinterpret_cast<LstmTcShared*>(sB + nK * kBTile);
+    float* sAcc = reinterpret_cast<float*>(sB + nK * kBTile);   // [NM][128][kLdAcc] staged accumulators
+    LstmTcShared* sh = reinterpret_cast<LstmTcShared*>(sAcc + NM * 128 * kLdAcc);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.y;
@@ -140,79 +97,79 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ 
 
     if (threadIdx.x == 0) {
         mbar_init(&sh->w_full, 1);
-        mbar_init(&sh->acc_ready, 1);
+        mbar_init(&sh->acc_ready, 128);
         mbar_init(&sh->h_ready, 32 * NEW);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < nK * kBTile / 4; i += blockDim.x) reinterpret_cast<float*>(sB)[i] = 0.f;
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sh->tmem_base)), "r"(64u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     fence_proxy_async_smem();
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = sh->tmem_base;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        if (threadIdx.x == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
             mbar_expect_tx(&sh->w_full, (uint32_t)(NM * nK * kATile));
             for (int m = 0; m < NM; ++m)
                 for (int kc = 0; kc < nK; ++kc)
                     tma_load_2d(sA + (m * nK + kc) * kATile, &mapW, &sh->w_full, kc * kKC, (dir * NM + m) * 128);
         }
-    } else if (warp == 1) {
-        // The whole warp walks the step loop and one elected lane issues: with `elect.sync` the compiler knows the tcgen05
-        // instructions are issued by a single converged lane and does not wrap each of them in its own election loop.
-        {
-            // UMMA instruction descriptor: D=F32 (1<<4), A=B=F16 (format 0), K-major, N=16, M=128
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(kNT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-            // The issuing thread is on the per-step critical path (a single thread pays ~6 cycles per dependent instruction):
-            // every descriptor is step-invariant, so build them once; only the low word changes along K (+2 per 32 bytes).
-            constexpr int kMaxKC = (ROWB == 128) ? 2 : 4;     // H <= 128
-            uint32_t da_lo[NM][kMaxKC], db_lo[kMaxKC];
-            const uint32_t d_hi = (uint32_t)(make_desc_kmajor<ROWB>(0) >> 32);
+        // MMA warpgroup.  Every descriptor is step-invariant, so they are built once; only the low bits change along K
+        // (+2 per 32 bytes) and with the 64-row half of a tile.
+        constexpr int kMaxKC = (ROWB == 128) ? 2 : 4;     // H <= 128
+        uint64_t da[NM][kMaxKC], db[kMaxKC];
+        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
 #pragma unroll
-            for (int kc = 0; kc < kMaxKC; ++kc) {
-                db_lo[kc] = (uint32_t)make_desc_kmajor<ROWB>(b0 + (uint32_t)(kc * kBTile));
+        for (int kc = 0; kc < kMaxKC; ++kc) {
+            db[kc] = make_desc_kmajor<ROWB>(b0 + (uint32_t)(kc * kBTile));
 #pragma unroll
-                for (int m = 0; m < NM; ++m) da_lo[m][kc] = (uint32_t)make_desc_kmajor<ROWB>(a0 + (uint32_t)((m * nK + kc) * kATile));
-            }
-            mbar_wait(&sh->w_full, 0);
-            for (int s = 1; s < p.steps; ++s) {
-                mbar_wait(&sh->h_ready, (uint32_t)((s - 1) & 1));
-                tcgen05_fence_after();
-                if (!elect_one()) continue;
-                LSTM_TRACE(0, s);
+            for (int m = 0; m < NM; ++m) da[m][kc] = make_desc_kmajor<ROWB>(a0 + (uint32_t)((m * nK + kc) * kATile));
+        }
+        float* const arow = sAcc + (warp * 16 + (lane >> 2)) * kLdAcc + 2 * (lane & 3);
+        mbar_wait(&sh->w_full, 0);
+        for (int s = 1; s < p.steps; ++s) {
+            mbar_wait(&sh->h_ready, (uint32_t)((s - 1) & 1));
+            LSTM_TRACE(0, s);
+            float d[NM][2][8];          // first written by the first wgmma of each chain (scale-d = 0)
+            wgmma_fence();
 #pragma unroll
-                for (int m = 0; m < NM; ++m) {
+            for (int m = 0; m < NM; ++m) {
+#pragma unroll
+                for (int hf = 0; hf < 2; ++hf) {
 #pragma unroll
                     for (int kc = 0; kc < kMaxKC; ++kc) {
                         if (kc < nK) {
 #pragma unroll
-                            for (int k = 0; k < ROWB / 32; ++k) {      // K = 16 fp16 = 32 B per UMMA
-                                if (kc == 0 && k == 0) umma_f16_lohi<false>(tmem_base + (uint32_t)(m * kNT), da_lo[m][kc], db_lo[kc], d_hi, idesc);
-                                else umma_f16_lohi<true>(tmem_base + (uint32_t)(m * kNT), da_lo[m][kc] + 2 * k, db_lo[kc] + 2 * k, d_hi, idesc);
-                            }
+                            for (int k = 0; k < ROWB / 32; ++k)        // K = 16 fp16 = 32 B per wgmma
+                                Wgmma<kNT, true, 0>::ss(d[m][hf], da[m][kc] + (uint64_t)(hf * ((64 * ROWB) >> 4) + 2 * k), db[kc] + 2 * k,
+                                                        (kc == 0 && k == 0) ? 0u : 1u);
                         }
                     }
                 }
-                umma_commit(&sh->acc_ready);
-                LSTM_TRACE(1, s);
             }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int m = 0; m < NM; ++m)
+#pragma unroll
+                for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) {
+                        float* r = arow + (m * 128 + hf * 64) * kLdAcc + 8 * j;
+                        *reinterpret_cast<float2*>(r) = make_float2(d[m][hf][4 * j], d[m][hf][4 * j + 1]);
+                        *reinterpret_cast<float2*>(r + 8 * kLdAcc) = make_float2(d[m][hf][4 * j + 2], d[m][hf][4 * j + 3]);
+                    }
+            mbar_arrive(&sh->acc_ready);
+            LSTM_TRACE(1, s);
         }
     } else {
-        // ===================================================== cell update (warps 2..2+NEW)
-        const int ew = warp - 2;
-        const int q = warp & 3;                          // TMEM lane quarter
+        // ===================================================== cell update (warps 4..4+NEW)
+        const int ew = warp - 4;
+        const int q = warp & 3;                          // 32-row quarter of every tile
         const int wp = ew >> 2;                          // which slice of the 16 sequences
         const int sub = lane / CPW;                      // gate slot inside the tile (0 for GPT=1)
         const int cell = q * CPW + (lane % CPW);
         const bool cell_ok = cell < H;
-        const int r = q * 32 + lane;                     // TMEM lane == gin column inside a tile
+        const int r = q * 32 + lane;                     // accumulator row == gin column inside a tile
         const int half = p.win_stride / 2;
         const int dpos = dir ? -1 : 1;
         const int pos0 = dir ? p.steps - 1 : 0;
@@ -321,7 +278,6 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ 
             if (ew == 0 && lane == 0) LSTM_TRACE(2, s);
             if (s > 0) {
                 mbar_wait(&sh->acc_ready, (uint32_t)((s - 1) & 1));
-                tcgen05_fence_after();
             }
             if (ew == 0 && lane == 0) LSTM_TRACE(3, s);
             float a[NM][kNS];
@@ -329,7 +285,12 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ 
             for (int m = 0; m < NM; ++m) {
                 uint32_t acc[kNS];
                 if (s > 0) {
-                    tmem_ld_n<kNS>(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * kNT + wp * kNS), acc);
+                    const uint32_t arow = smem_u32(sAcc + (m * 128 + r) * kLdAcc + wp * kNS);
+#pragma unroll
+                    for (int i = 0; i < kNS; i += 4) {
+                        const float4 v = lds128(arow + 4u * i);
+                        acc[i] = __float_as_uint(v.x); acc[i + 1] = __float_as_uint(v.y); acc[i + 2] = __float_as_uint(v.z); acc[i + 3] = __float_as_uint(v.w);
+                    }
                 } else {
 #pragma unroll
                     for (int i = 0; i < kNS; ++i) acc[i] = 0u;
@@ -374,16 +335,10 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ 
             if (ew == 0 && lane == 0) LSTM_TRACE(5, s);
             if (s + 1 < p.steps) {
                 fence_proxy_async_smem();                // generic-proxy stores of h -> visible to the tensor core
-                tcgen05_fence_before();
                 mbar_arrive(&sh->h_ready);
             }
             if (ew == 0 && lane == 0) LSTM_TRACE(6, s);
         }
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(64u) : "memory");
     }
 }
 
@@ -392,11 +347,11 @@ static void lstm_tc_go(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMa
                        const aero_lstm_params& p, int nK) {
     if (p.flags & AERO_TG_A_F16) {          // gate pre-activations stored in FP16
         cudaFuncSetAttribute(lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, __half><<<grid, 64 + 32 * NEW, smem, st>>>(mW, static_cast<const __half*>(gin), bias_pad,
+        lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, __half><<<grid, 128 + 32 * NEW, smem, st>>>(mW, static_cast<const __half*>(gin), bias_pad,
                                                                                               static_cast<TO*>(hout), p, nK);
     } else {
         cudaFuncSetAttribute(lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, float><<<grid, 64 + 32 * NEW, smem, st>>>(mW, static_cast<const float*>(gin), bias_pad,
+        lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, float><<<grid, 128 + 32 * NEW, smem, st>>>(mW, static_cast<const float*>(gin), bias_pad,
                                                                                              static_cast<TO*>(hout), p, nK);
     }
 }
@@ -405,7 +360,7 @@ int lstm_tc_launch(const void* gin, const float* bias_pad, const void* whh_r, vo
                    cudaStream_t st) {
     const int H = p.H;
     if (H % 4 || H <= 32 || H > 128) {
-        set_error("aero_lstm_rec_fwd(tcgen05): hidden size %d unsupported (multiple of 4 in (32, 128])", H);
+        set_error("aero_lstm_rec_fwd(wgmma): hidden size %d unsupported (multiple of 4 in (32, 128])", H);
         return AERO_ERR_UNSUPPORTED;
     }
     static int num_sms = 0;
@@ -419,10 +374,10 @@ int lstm_tc_launch(const void* gin, const float* bias_pad, const void* whh_r, vo
     const int nM = 4 / gpt;
     const int Kp = ((H + 63) / 64) * 64;                 // the host pads W_hh rows to a multiple of 64 fp16 (128 bytes)
     // Small CTAs (8 sequences) whenever all of them fit on the GPU at once at the co-residency they allow: twice the SMs
-    // busy and, where two or three share an SM, one CTA's barrier / MMA latency hides behind another's cell update.
-    // GPT = 1 keeps W_hh in 32-column SWIZZLE_64B chunks then (no K padding; two CTAs per SM up to H = 96).
+    // busy and, where two share an SM (GPT = 2), one CTA's barrier / MMA latency hides behind another's cell update.
+    // GPT = 1 keeps W_hh in 32-column SWIZZLE_64B chunks then (no K padding).
     const int knob = lstm_seq_knob();
-    const bool small = knob ? knob == 8 : (int64_t)cdiv(n_seq, 8) * 2 <= (int64_t)num_sms * (gpt == 1 ? (H <= 96 ? 2 : 1) : 3);
+    const bool small = knob ? knob == 8 : (int64_t)cdiv(n_seq, 8) * 2 <= (int64_t)num_sms * (gpt == 1 ? 1 : 2);
     const int rowb = (gpt == 1 && small) ? 64 : 128;
     const int kc_elems = rowb / 2;
     const int nK = (H + kc_elems - 1) / kc_elems;
@@ -432,14 +387,14 @@ int lstm_tc_launch(const void* gin, const float* bias_pad, const void* whh_r, vo
     uint32_t box[2] = {(uint32_t)kc_elems, 128};
     int rc = encode_map(&mW, whh_r, 2, dims, strides, box, rowb == 64 ? 2 : 0, 2);
     if (rc != AERO_OK) return rc;
-    const size_t smem = (size_t)nM * nK * 128 * rowb + (size_t)nK * kNT * rowb + sizeof(LstmTcShared) + 1024;
+    const size_t smem = (size_t)nM * nK * 128 * rowb + (size_t)nK * kNT * rowb + (size_t)nM * 128 * kLdAcc * 4 + sizeof(LstmTcShared) + 1024;
     if (smem > 227 * 1024) {
-        set_error("aero_lstm_rec_fwd(tcgen05): hidden size %d needs %zu bytes of shared memory", H, smem);
+        set_error("aero_lstm_rec_fwd(wgmma): hidden size %d needs %zu bytes of shared memory", H, smem);
         return AERO_ERR_UNSUPPORTED;
     }
     const int64_t max_rows = (int64_t)n_seq * p.steps > (int64_t)p.rows * p.T ? (int64_t)n_seq * p.steps : (int64_t)p.rows * p.T;
     if ((max_rows + p.steps) * (8ll * H) >= (1ll << 31)) {
-        set_error("aero_lstm_rec_fwd(tcgen05): problem too large for 32-bit offsets (%lld rows)", (long long)max_rows);
+        set_error("aero_lstm_rec_fwd(wgmma): problem too large for 32-bit offsets (%lld rows)", (long long)max_rows);
         return AERO_ERR_UNSUPPORTED;
     }
     dim3 grid(cdiv(n_seq, small ? 8 : kNT), 2);
@@ -450,14 +405,14 @@ int lstm_tc_launch(const void* gin, const float* bias_pad, const void* whh_r, vo
         else lstm_tc_go<GPT, NEW, SEQ, ROWB, MINB, float>(grid, smem, st, mW, gin, bias_pad, hout, p, nK);      \
     } while (0)
     if (gpt == 1) {
-        if (small) AERO_LSTM_GO(1, 8, 8, 64, 2);
+        if (small) AERO_LSTM_GO(1, 8, 8, 64, 1);
         else AERO_LSTM_GO(1, 16, 16, 128, 1);
     } else {
-        if (small) AERO_LSTM_GO(2, 8, 8, 128, 3);
+        if (small) AERO_LSTM_GO(2, 8, 8, 128, 2);
         else AERO_LSTM_GO(2, 8, 16, 128, 2);
     }
 #undef AERO_LSTM_GO
-    return check_launch("aero_lstm_rec_fwd(tcgen05)");
+    return check_launch("aero_lstm_rec_fwd(wgmma)");
 }
 
 }  // namespace aero

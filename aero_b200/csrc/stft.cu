@@ -1,4 +1,4 @@
-// Fused STFT / iSTFT kernels for sm_100a.
+// Fused STFT / iSTFT kernels for sm_90a.
 //
 // aero_stft_fwd  : reflect pad + framing + window + real FFT (N/2-point complex FFT in shared
 //                  memory + split post-pass) + n_fft^-1/2 + Nyquist drop + strided (channels-last

@@ -65,7 +65,7 @@ extern "C" int aero_stft_loss_bwd(const float* z_est, const float* z_ref, const 
     AERO_REQUIRE(z_est && z_ref && sums && g_est && B >= 1 && bins == n_fft / 2 + 1 && frames >= 1, "aero_stft_loss_bwd: bad argument");
     const int64_t n = (int64_t)B * bins * frames;
     int blocks = (int)((n + 256 * 8 - 1) / (256 * 8));
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     stft_loss_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float2*>(z_est), reinterpret_cast<const float2*>(z_ref), sums,
                                                                   reinterpret_cast<float2*>(g_est), n, (float)n_fft, bins, frames, c_sc, c_mag);
@@ -78,7 +78,7 @@ extern "C" int aero_stft_loss_fwd(const float* z_est, const float* z_ref, double
     AERO_REQUIRE(z_est && z_ref && sums && B >= 1 && bins >= 1 && frames >= 1 && n_fft >= 2, "aero_stft_loss_fwd: bad argument");
     const int64_t n = (int64_t)B * bins * frames;
     int blocks = (int)((n + 256 * 8 - 1) / (256 * 8));
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     stft_loss_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float2*>(z_est), reinterpret_cast<const float2*>(z_ref),
                                                               sums, n, (float)n_fft);

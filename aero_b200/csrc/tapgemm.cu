@@ -1,4 +1,4 @@
-// aero_tapgemm_fwd: validation + dispatch (fp32 SIMT tiles, or TF32 tcgen05 tiles when eligible).
+// aero_tapgemm_fwd: validation + dispatch (fp32 SIMT tiles, or TF32 wgmma tiles when eligible).
 #include "tapgemm.cuh"
 
 
@@ -20,7 +20,7 @@ extern "C" int aero_tapgemm_fwd(const void* a1, const void* a2, const void* w, c
         AERO_REQUIRE(p.kt == 1 && p.kf % p.stride_f == 0, "aero_tapgemm_fwd: transposed conv needs kt=1 and kf %% stride == 0");
         ntaps = p.kf / p.stride_f;
     } else if (p.mode == AERO_TAPS_MIX) {
-        AERO_REQUIRE(p.precision == 1 || p.precision == 2, "aero_tapgemm_fwd: AERO_TAPS_MIX exists on the tcgen05 path only (precision 1 / 2)");
+        AERO_REQUIRE(p.precision == 1 || p.precision == 2, "aero_tapgemm_fwd: AERO_TAPS_MIX exists on the wgmma path only (precision 1 / 2)");
         ntaps = 1;
     } else {
         set_error("aero_tapgemm_fwd: mode=%d", p.mode);
@@ -61,7 +61,7 @@ extern "C" int aero_tapgemm_fwd(const void* a1, const void* a2, const void* w, c
                  "aero_tapgemm_fwd: precision 1 reads fp32 sources, precision 2 FP16 sources (flags=%d)", p.flags);
     if (p.precision >= 1) {
         if (!tapgemm_tc_eligible(p)) {
-            set_error("aero_tapgemm_fwd: tcgen05 path requested for a shape the tcgen05 path does not take (N=%d K=%d)", p.N, p.C1 + p.C2);
+            set_error("aero_tapgemm_fwd: wgmma path requested for a shape the wgmma path does not take (N=%d K=%d)", p.N, p.C1 + p.C2);
             return AERO_ERR_UNSUPPORTED;
         }
         AERO_REQUIRE((p.C1 == 0 || al16(a1)) && (p.C2 == 0 || al16(a2)), "aero_tapgemm_fwd: TMA sources must be 16-byte aligned");

@@ -1,5 +1,6 @@
 // Shared argument block of the tap-GEMM implementations.
 #pragma once
+#include <cuda.h>
 #include "common.cuh"
 
 namespace aero {
@@ -21,13 +22,30 @@ struct TapGemmArgs {
     int vec_a;        // 16-byte loads of A are legal
     int vec_o;        // 16-byte stores legal
     int vec_o8;       // FP16 outputs: rows are 16-byte aligned in units of 8 halves (direct lane-per-row epilogue)
-    // tcgen05 path: exact division of tile indices (< 2^31) by n_tiles, tiles_t, F_out:  q = (n * mul) >> shr
+    // tensor-core path: exact division of tile indices (< 2^31) by n_tiles, tiles_t, F_out:  q = (n * mul) >> shr
     uint32_t dv_mul[3], dv_shr[3];
     int direct_f16;   // FP16 outputs: same choice
     int direct_f32;   // fp32 outputs: direct lane-per-row epilogue instead of the shared-memory transpose
     int last_tile;    // tiles_total - 1 (reverse walk)
-    int grouped_bn;   // tiles with BN <= this use the two-group epilogue
 };
+// tensor-core path: tile geometry and the fixed part of a CTA's shared memory, shared by the kernel and its launcher
+constexpr int kBM = 128;
+constexpr int kMaxStages = 8;
+constexpr int kMaxBN = 128;             // widest wgmma N used; wider layers take several n-tiles
+constexpr int kEpiWarps = 8;             // the two consumer warpgroups: two warps per 32-row quarter, alternating 16-column chunks
+constexpr int kThreads = 128 + 32 * kEpiWarps;
+constexpr int kATileBytes = kBM * 128;   // 16 KB
+
+struct TcShared {
+    uint64_t full[kMaxStages];
+    uint64_t empty[kMaxStages];
+    float stats[kEpiWarps][8][2];   // [epilogue warp][group slot][sum, sumsq]: fixed-order reduction, run-to-run deterministic
+    float part[kEpiWarps][4][2];    // per-warp scratch for the fixed-order flush of the coalesced epilogue
+    alignas(16) float stage[kEpiWarps][32][20];   // per-warp transpose buffer (16 columns): lane-per-row -> row-contiguous stores
+};
+
+// a tensor-core tap-GEMM kernel: (A1 map, A2 map, W map, args, stages, n-tiles, tiles)
+using KernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TapGemmArgs, int, int, int);
 int tapgemm_simt_launch(const TapGemmArgs& g, cudaStream_t st);
 int tapgemm_tc_launch(const TapGemmArgs& g, cudaStream_t st);
 bool tapgemm_tc_eligible(const aero_tapgemm_params& p);

@@ -1,5 +1,5 @@
 // Tap-GEMM, fp32 SIMT implementation (exact-fp32 accumulate; the parity anchor and the fallback
-// for shapes the tcgen05 path does not take).  See include/aero_b200.h for the operator contract.
+// for shapes the wgmma path does not take).  See include/aero_b200.h for the operator contract.
 //
 // Tile: BM pixels (consecutive t inside one (b, f_out) row) x BN output columns, K consumed in
 // chunks of 16 channels per tap; 256 threads, TM x TN register tile per thread.
@@ -482,11 +482,11 @@ static int tapgemm_simt_launch_t(const TapGemmArgs& g, cudaStream_t st) {
         const int n_a = a_hi - a_lo + 1;
         const int64_t npix = (int64_t)p.B * n_a * p.T;
         int blocks = (int)((npix + 255) / 256);
-        if (blocks > 148 * 16) blocks = 148 * 16;
+        if (blocks > 132 * 16) blocks = 132 * 16;
         tapgemm_thin_convt_kernel<TA, TO><<<blocks, 256, smem, st>>>(a, a_lo, n_a);
         return check_launch("aero_tapgemm_fwd(thin-convt)");
     }
-    if (plain && p.N <= kThinN && g.vec_a && (int64_t)nslab * (p.C1 + p.C2) >= 1024 && (int64_t)p.B * p.F_out * p.T <= 148 * 64) {
+    if (plain && p.N <= kThinN && g.vec_a && (int64_t)nslab * (p.C1 + p.C2) >= 1024 && (int64_t)p.B * p.F_out * p.T <= 132 * 64) {
         const int64_t npix = (int64_t)p.B * p.F_out * p.T;           // long dot products, few pixels: a warp per pixel
         tapgemm_thin_n_warp_kernel<TA, TO><<<(unsigned)cdiv(npix, (int64_t)8), 256, 0, st>>>(a);
         return check_launch("aero_tapgemm_fwd(thin-n, warp per pixel)");
@@ -496,7 +496,7 @@ static int tapgemm_simt_launch_t(const TapGemmArgs& g, cudaStream_t st) {
         cudaFuncSetAttribute(tapgemm_thin_n_kernel<TA, TO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         const int64_t npix = (int64_t)p.B * p.F_out * p.T;
         int blocks = (int)((npix + 255) / 256);
-        if (blocks > 148 * 16) blocks = 148 * 16;
+        if (blocks > 132 * 16) blocks = 132 * 16;
         tapgemm_thin_n_kernel<TA, TO><<<blocks, 256, smem, st>>>(a);
         return check_launch("aero_tapgemm_fwd(thin-n)");
     }
@@ -505,7 +505,7 @@ static int tapgemm_simt_launch_t(const TapGemmArgs& g, cudaStream_t st) {
         const int ppp = 256 / (p.N / 4);
         const int64_t npix = (int64_t)p.B * p.F_out * p.T;
         int blocks = (int)((npix + (int64_t)ppp * 8 - 1) / ((int64_t)ppp * 8));
-        if (blocks > 148 * 32) blocks = 148 * 32;
+        if (blocks > 132 * 32) blocks = 132 * 32;
         if (blocks < 1) blocks = 1;
         tapgemm_thin_k_kernel<TA, TO><<<blocks, 256, 0, st>>>(a);
         return check_launch("aero_tapgemm_fwd(thin-k)");

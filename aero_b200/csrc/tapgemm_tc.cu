@@ -1,673 +1,21 @@
-// Tap-GEMM on the 5th-generation tensor cores (sm_100a): TMA -> shared memory -> tcgen05.mma (kind::f16 / kind::tf32, fp32
-// accumulate in TMEM) -> tcgen05.ld epilogue.  Implicit GEMM, im2col-free: every tap of a convolution is a shifted TMA box
-// of the channels-last activation tensor; image borders, channel tails and the K tail are TMA out-of-bounds zero fill.
-//
-//   A tile : 128 pixels (consecutive t of one (b, f) row) x 128 bytes of channels = 128 rows, SWIZZLE_128B
-//   B tile : BN output columns x 128 bytes of channels (weights stored K-major [slab][N][K]) = BN rows
-//   D      : 128 lanes x BN fp32 columns of TMEM, two buffers (the epilogue of tile i overlaps the main loop of tile i+1)
-// Persistent CTAs (one or two per SM) of 320 threads: warp 0 = TMA producer (runs ahead across tiles), warp 1 = TMEM allocator +
-// MMA issue by one elected lane, warps 2..9 = epilogue.  STAGES-deep mbarrier ring between producer and MMA; tcgen05.commit
-// frees a stage / publishes an accumulator buffer.
-//
-// Operand kinds: kind::tf32 (fp32 storage, 32 channels per 128-byte row, UMMA_K = 8) or kind::f16 (FP16 storage, 64 channels
-// per row, UMMA_K = 16): the shared-memory image is identical in bytes (128 rows x 128 B per k-block, four UMMAs of 32 B along
-// K), so one kernel serves both.  FP16 has TF32's 10-bit mantissa at half the HBM bytes and twice the tensor-core rate.
-// Outputs are fp32 or FP16 independently of the operand kind.
-//
-// TF32 operands are read as fp32 bit patterns with the low 13 mantissa bits ignored by the tensor core,
-// so producers round activations to TF32 (round-to-nearest) when they store them and the host
-// rounds the weights when it packs them: truncation would bias every dot product low.
+// Host side of the tensor-core tap-GEMM: TMA descriptors, tile-width choice, launch.  The kernel is in tapgemm_tc_kernel.cuh.
 #include <cuda.h>
 #include <mutex>
 #include <unordered_map>
 #include <string>
 #include <cstring>
 #include <cstdlib>
-#include <type_traits>
 
 #include "tapgemm.cuh"
 #include "tc_common.cuh"
 
-#ifdef AERO_TC_TRACE
-// tuning aid (tools/tc_trace.py builds a separate library with this flag): clock64 stamps of CTA 0's pipeline events
-__device__ long long g_tc_trace[256 * 8];
-#define AERO_TRACE(slot, local) do { if (blockIdx.x == 0 && (local) < 256) g_tc_trace[(local) * 8 + (slot)] = clock64(); } while (0)
-extern "C" int aero_debug_tc_trace(long long* host) {
-    return cudaMemcpyFromSymbol(host, g_tc_trace, sizeof(g_tc_trace)) == cudaSuccess ? 0 : -1;
-}
-#else
-#define AERO_TRACE(slot, local) do { } while (0)
-#endif
-
 namespace aero {
 
-constexpr int kBM = 128;
-template <bool F16A> struct OperandKind { static constexpr int kBK = F16A ? 64 : 32; };   // elements per 128-byte swizzle row
-constexpr int kMaxStages = 8;
-constexpr int kEpiWarps = 8;             // two per TMEM lane quarter, alternating 16-column chunks
-constexpr int kThreads = 64 + 32 * kEpiWarps;
-constexpr int kATileBytes = kBM * 128;   // 16 KB
+KernelFn tapgemm_tc_kernels_bn32(bool f16a, bool f16o, int amode, bool res, bool stats);
+KernelFn tapgemm_tc_kernels_bn64(bool f16a, bool f16o, int amode, bool res, bool stats);
+KernelFn tapgemm_tc_kernels_bn96(bool f16a, bool f16o, int amode, bool res, bool stats);
+KernelFn tapgemm_tc_kernels_bn128(bool f16a, bool f16o, int amode, bool res, bool stats);
 
-struct TcShared {
-    uint64_t full[kMaxStages];
-    uint64_t empty[kMaxStages];
-    uint64_t acc_full[2];      // MMA -> epilogue, one per TMEM accumulator buffer
-    uint64_t acc_empty[2];     // epilogue -> MMA
-    uint32_t tmem_base;
-    float stats[kEpiWarps][8][2];   // [epilogue warp][group slot][sum, sumsq]: fixed-order reduction, run-to-run deterministic
-    float part[kEpiWarps][4][2];    // per-warp scratch for the fixed-order flush of the coalesced epilogue
-    alignas(16) float stage[kEpiWarps][32][20];   // per-warp transpose buffer (16 columns): lane-per-row -> row-contiguous stores
-};
-
-// number of (tap, source, channel-chunk) iterations and their enumeration, shared by all roles
-struct TapIter {
-    int fi, dt, slab;
-};
-__device__ __forceinline__ bool tap_geometry(const aero_tapgemm_params& p, int tap, int fo, TapIter& it) {
-    if (p.mode == AERO_TAPS_CONV) {
-        const int jf = tap / p.kt, jt = tap - jf * p.kt;
-        it.fi = fo * p.stride_f + jf - p.pad_f;
-        it.dt = jt * p.dil_t - p.pad_t;
-        it.slab = tap;
-    } else {
-        const int fof = fo + p.f_out_offset;
-        it.fi = fof / p.stride_f - tap;
-        it.dt = 0;
-        it.slab = fof % p.stride_f + tap * p.stride_f;
-    }
-    return it.fi >= 0 && it.fi < p.F_in;
-}
-
-struct TileCoord {
-    int b, fo, t0, n0, n_iters;
-};
-// exact n / d for n < 2^31 (Granlund-Montgomery round-up multiplier, set up by the host): three instructions instead of ~25
-__device__ __forceinline__ int fast_div(int n, uint32_t mul, uint32_t shr) {
-    return (int)(((uint64_t)(uint32_t)n * mul) >> shr);
-}
-// number of taps whose input row exists (time-axis borders are TMA zero fill and always count)
-__device__ __forceinline__ int valid_taps(const aero_tapgemm_params& p, int fo, int ntaps) {
-    if (p.mode == AERO_TAPS_CONV) {
-        const int base = fo * p.stride_f - p.pad_f;                    // fi = base + jf
-        const int lo = max(0, -base), hi = min(p.kf - 1, p.F_in - 1 - base);
-        return max(0, hi - lo + 1) * p.kt;
-    }
-    const int a = (fo + p.f_out_offset) / p.stride_f;                  // fi = a - tap
-    const int lo = max(0, a - p.F_in + 1), hi = min(ntaps - 1, a);
-    return max(0, hi - lo + 1);
-}
-// tile order: the n-tiles of one pixel tile are adjacent, so CTAs working at the same time share the A operand in L2
-__device__ __forceinline__ TileCoord tile_coord(const TapGemmArgs& g, int tile, int n_tiles, int BN, int nch1, int nch2) {
-    const aero_tapgemm_params& p = g.p;
-    TileCoord c;
-    if (p.flags & AERO_TG_REVERSE) tile = g.last_tile - tile;       // walk from the end: see AERO_TG_REVERSE
-    const int mt = fast_div(tile, g.dv_mul[0], g.dv_shr[0]), nt = tile - mt * n_tiles;
-    const int row = fast_div(mt, g.dv_mul[1], g.dv_shr[1]), tt = mt - row * g.tiles_t;
-    c.b = fast_div(row, g.dv_mul[2], g.dv_shr[2]);
-    c.fo = row - c.b * p.F_out;
-    c.t0 = tt * kBM;
-    c.n0 = nt * BN;
-    c.n_iters = (p.mode == AERO_TAPS_MIX) ? nch1 : valid_taps(p, c.fo, g.ntaps) * (nch1 + nch2);
-    return c;
-}
-
-// Coalesced epilogue, specialised at compile time (AMODE: 0 none, 1 GELU, 2 ReLU, 3 GLU; RES: residual add; STATS).
-// Stage A: this thread's 16 accumulator columns of its row -> bias -> activation / GLU -> row `lane` of the per-warp
-// staging tile.  Stage B: the warp walks the tile so that consecutive lanes hold consecutive float4s of one output row
-// (residual loads and stores are whole 32-byte sectors of one row), adds the row-wise terms, rounds, accumulates statistics.
-template <int AMODE>
-__device__ __forceinline__ void epilogue_stage_a(const uint32_t (&r)[16], uint32_t stg_row, uint32_t sbias) {
-    // stg_row: shared-space address of this lane's staging row; sbias: shared-space address of this chunk's 16 bias values
-    float4 bv[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) bv[j] = lds128(sbias + 16 * j);
-#pragma unroll
-    for (int j = 0; j < 16; j += 4) {
-        float v[4] = {__uint_as_float(r[j]) + bv[j / 4].x, __uint_as_float(r[j + 1]) + bv[j / 4].y,
-                      __uint_as_float(r[j + 2]) + bv[j / 4].z, __uint_as_float(r[j + 3]) + bv[j / 4].w};
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            if (AMODE == 1) v[u] = gelu_exact(v[u]);
-            else if (AMODE == 2) v[u] = fmaxf(v[u], 0.f);
-        }
-        if (AMODE == 3) {
-            sts64(stg_row + (j / 2) * 4, v[0] * sigmoid_f(v[1]), v[2] * sigmoid_f(v[3]));
-        } else {
-            sts128(stg_row + j * 4, make_float4(v[0], v[1], v[2], v[3]));
-        }
-    }
-}
-
-template <int AMODE, bool RES, bool STATS, typename TO>
-__device__ __forceinline__ void epilogue_fast_tile(TcShared* sh, const TapGemmArgs& g, const TileCoord& tc, uint32_t tacc, int BN, int q,
-                                                   int ew, int lane, int Nout, int gw, int c_start, int c_step, uint32_t sbias) {
-    const aero_tapgemm_params& p = g.p;
-    constexpr int CNT = (AMODE == 3) ? 8 : 16;          // staged output columns per 16 accumulator columns
-    constexpr int LPR = CNT / 4;                         // lanes per row (one float4 each)
-    constexpr int RPI = 32 / LPR;                        // rows per pass
-    const uint32_t stg = smem_u32(&sh->stage[ew][0][0]);       // [32][20] floats, addressed in the shared window
-    const bool rnd = (p.flags & 1) && sizeof(TO) == 4;
-    float sa = 1.f, sb = 0.f;
-    if (g.samp_affine) { sa = g.samp_affine[2 * tc.b]; sb = g.samp_affine[2 * tc.b + 1]; }
-    const int cq = lane % LPR, ro = lane / LPR;
-    const int row0 = tc.t0 + q * 32;                     // first output row (t) of this warp's lane quarter
-    const int rows = min(32, p.T - row0);                // valid rows (<= 0: nothing to store)
-    const int g_lo = ((AMODE == 3) ? tc.n0 >> 1 : tc.n0) / gw;
-    TO* const obase = static_cast<TO*>(g.out) + (int64_t)tc.b * p.o_sb + (int64_t)tc.fo * p.o_sf + (int64_t)row0 * p.o_st;
-    const TO* const rbase = RES ? static_cast<const TO*>(g.residual) + (int64_t)tc.b * p.r_sb + (int64_t)tc.fo * p.r_sf + (int64_t)row0 * p.r_st : nullptr;
-    const float* const adp = g.addend_fn ? g.addend_fn + (int64_t)tc.fo * Nout : nullptr;
-    for (int c0 = c_start; c0 < BN; c0 += c_step) {      // split mode: the two warps of a lane quarter alternate 16-column chunks
-        const int nb = tc.n0 + c0;
-        if (nb >= p.N) break;
-        uint32_t r[16];
-        if (tc.n_iters > 0) {
-            tmem_ld16(tacc + (uint32_t)c0, r);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) r[j] = 0u;
-        }
-        epilogue_stage_a<AMODE>(r, stg + (uint32_t)lane * 80u, sbias + (uint32_t)nb * 4u);
-        __syncwarp();
-        const int no0 = (AMODE == 3) ? nb >> 1 : nb;
-        const int nn = no0 + 4 * cq;
-        float ls = 0.f, lq = 0.f;
-        if (nn < Nout) {                                 // Nout % 4 == 0 (vec_o)
-            float4 ad = make_float4(0.f, 0.f, 0.f, 0.f);
-            const bool has_ad = adp != nullptr, affine = g.samp_affine != nullptr;
-            if (has_ad) ad = *reinterpret_cast<const float4*>(adp + nn);
-            uint32_t sp = stg + (uint32_t)(ro * 80 + cq * 16);
-            TO* op = obase + (int64_t)ro * p.o_st + nn;
-            const TO* rp = RES ? rbase + (int64_t)ro * p.r_st + nn : nullptr;
-            const int64_t ostep = (int64_t)RPI * p.o_st, rstep = (int64_t)RPI * p.r_st;
-#pragma unroll 2
-            for (int rr = ro; rr < rows; rr += RPI) {
-                float4 x = lds128(sp);
-                sp += RPI * 80;
-                if (has_ad) { x.x += ad.x; x.y += ad.y; x.z += ad.z; x.w += ad.w; }
-                if (RES) {
-                    const float4 rs = ld4(rp);
-                    x.x += rs.x; x.y += rs.y; x.z += rs.z; x.w += rs.w;
-                    rp += rstep;
-                }
-                if (affine) { x.x = fmaf(x.x, sa, sb); x.y = fmaf(x.y, sa, sb); x.z = fmaf(x.z, sa, sb); x.w = fmaf(x.w, sa, sb); }
-                if (rnd) { x.x = round_tf32_rna(x.x); x.y = round_tf32_rna(x.y); x.z = round_tf32_rna(x.z); x.w = round_tf32_rna(x.w); }
-                if (STATS) {
-                    if (sizeof(TO) == 2) {               // statistics describe the values as stored (FP16 pre-normalisation tensors)
-                        x.x = stored(x.x, op); x.y = stored(x.y, op); x.z = stored(x.z, op); x.w = stored(x.w, op);
-                    }
-                    ls += (x.x + x.y) + (x.z + x.w);
-                    lq += (x.x * x.x + x.y * x.y) + (x.z * x.z + x.w * x.w);
-                }
-                st4(op, x);
-                op += ostep;
-            }
-        }
-        if (STATS) {
-            const int g_first = no0 / gw, g_last = (min(no0 + CNT, Nout) - 1) / gw;
-            if (g_first == g_last) {
-                // the whole chunk is one group: plain warp reduction (fixed xor order -> deterministic)
-                const float a = warp_sum(ls), c = warp_sum(lq);
-                if (lane == 0) { sh->stats[ew][g_first - g_lo][0] += a; sh->stats[ew][g_first - g_lo][1] += c; }
-            } else {
-                // lanes with the same column quad first, then a fixed-order pass over the quads by lane 0
-                for (int o = LPR; o < 32; o <<= 1) { ls += __shfl_xor_sync(0xffffffffu, ls, o); lq += __shfl_xor_sync(0xffffffffu, lq, o); }
-                if (lane < LPR) { sh->part[ew][lane][0] = ls; sh->part[ew][lane][1] = lq; }
-                __syncwarp();
-                if (lane == 0) {
-                    for (int u = 0; u < LPR; ++u) {
-                        const int nq = no0 + 4 * u;
-                        if (nq < Nout) {
-                            sh->stats[ew][nq / gw - g_lo][0] += sh->part[ew][u][0];
-                            sh->stats[ew][nq / gw - g_lo][1] += sh->part[ew][u][1];
-                        }
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    }
-}
-
-// Direct epilogue: a lane's 16 accumulator columns of its row are 32 (FP16) or 64 (fp32) contiguous bytes -- whole sectors --
-// so the row is written straight from registers with 16-byte stores and no shared-memory transpose.  Everything is unrolled
-// and independent (bias / residual / addend loads issue together), which is what the HBM-bound layers need: with one or two
-// warps per scheduler the epilogue is a latency chain, not a throughput problem.
-template <int AMODE, bool RES, bool STATS, typename TO>
-__device__ __forceinline__ void epilogue_direct(TcShared* sh, const TapGemmArgs& g, const TileCoord& tc, uint32_t tacc, int BN, int q, int ew,
-                                                int lane, int Nout, int gw, int c_start, int c_step, uint32_t sbias) {
-    const aero_tapgemm_params& p = g.p;
-    constexpr int CNT = (AMODE == 3) ? 8 : 16;          // output columns per 16 accumulator columns
-    constexpr bool F16 = sizeof(TO) == 2;
-    const int t = tc.t0 + q * 32 + lane;
-    const bool row_ok = t < p.T;
-    TO* const orow = static_cast<TO*>(g.out) + (int64_t)tc.b * p.o_sb + (int64_t)tc.fo * p.o_sf + (int64_t)t * p.o_st;
-    const TO* const rrow = RES ? static_cast<const TO*>(g.residual) + (int64_t)tc.b * p.r_sb + (int64_t)tc.fo * p.r_sf + (int64_t)t * p.r_st : nullptr;
-    const float* const adp = g.addend_fn ? g.addend_fn + (int64_t)tc.fo * Nout : nullptr;
-    float sa = 1.f, sb = 0.f;
-    const bool affine = g.samp_affine != nullptr;
-    if (affine) { sa = g.samp_affine[2 * tc.b]; sb = g.samp_affine[2 * tc.b + 1]; }
-    const bool rnd = (p.flags & 1) && !F16;
-    const int g_lo = ((AMODE == 3) ? tc.n0 >> 1 : tc.n0) / gw;
-    int cur_g = -1;                                      // statistics: running group (warp-uniform), flushed when it changes
-    float ssum = 0.f, ssq = 0.f;
-    for (int c0 = c_start; c0 < BN; c0 += c_step) {
-        const int nb = tc.n0 + c0;
-        if (nb >= p.N) break;
-        uint32_t r[16];
-        if (tc.n_iters > 0) {
-            tmem_ld16(tacc + (uint32_t)c0, r);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) r[j] = 0u;
-        }
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        {
-            float4 bv[4];                                // bias lives in shared memory (zero padded): broadcast reads, no L1 misses
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bv[j] = lds128(sbias + (uint32_t)nb * 4u + 16u * j);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { v[4 * j] += bv[j].x; v[4 * j + 1] += bv[j].y; v[4 * j + 2] += bv[j].z; v[4 * j + 3] += bv[j].w; }
-        }
-        float o[CNT];
-        if (AMODE == 3) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = v[2 * j] * sigmoid_f(v[2 * j + 1]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) o[j] = (AMODE == 1) ? gelu_exact(v[j]) : (AMODE == 2) ? fmaxf(v[j], 0.f) : v[j];
-        }
-        const int no0 = (AMODE == 3) ? nb >> 1 : nb;
-        const int n_ok = min(CNT, Nout - no0);           // valid output columns of this chunk (a multiple of 4; 8 for FP16: host check)
-        if (row_ok) {
-            if (adp) {
-#pragma unroll
-                for (int j = 0; j < CNT; j += 4)
-                    if (j < n_ok) {
-                        const float4 a = __ldg(reinterpret_cast<const float4*>(adp + no0 + j));
-                        o[j] += a.x; o[j + 1] += a.y; o[j + 2] += a.z; o[j + 3] += a.w;
-                    }
-            }
-            if (RES) {
-#pragma unroll
-                for (int j = 0; j < CNT; j += 4)
-                    if (j < n_ok) {
-                        const float4 a = ld4(rrow + no0 + j);
-                        o[j] += a.x; o[j + 1] += a.y; o[j + 2] += a.z; o[j + 3] += a.w;
-                    }
-            }
-            if (affine) {
-#pragma unroll
-                for (int j = 0; j < CNT; ++j) o[j] = fmaf(o[j], sa, sb);
-            }
-            if (rnd) {
-#pragma unroll
-                for (int j = 0; j < CNT; ++j) o[j] = round_tf32_rna(o[j]);
-            }
-            if (F16 && STATS) {                          // statistics describe the values as stored
-#pragma unroll
-                for (int j = 0; j < CNT; ++j) o[j] = stored(o[j], orow);
-            }
-            if (F16) {
-#pragma unroll
-                for (int j = 0; j < CNT; j += 8)
-                    if (j < n_ok) {
-                        uint4 u;
-                        u.x = pack_half2_sat(o[j], o[j + 1]); u.y = pack_half2_sat(o[j + 2], o[j + 3]);
-                        u.z = pack_half2_sat(o[j + 4], o[j + 5]); u.w = pack_half2_sat(o[j + 6], o[j + 7]);
-                        *reinterpret_cast<uint4*>(orow + no0 + j) = u;
-                    }
-            } else {
-#pragma unroll
-                for (int j = 0; j < CNT; j += 4)
-                    if (j < n_ok) *reinterpret_cast<float4*>(orow + no0 + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-            }
-        }
-        if (STATS) {
-            // group width is a multiple of 4 (host check), so every column quad lies in one group
-#pragma unroll
-            for (int j = 0; j < CNT; j += 4) {
-                if (j < n_ok) {
-                    const int gi = (no0 + j) / gw;
-                    if (gi != cur_g) {
-                        if (cur_g >= 0) {
-                            const float a = warp_sum(ssum), c = warp_sum(ssq);
-                            if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] += a; sh->stats[ew][cur_g - g_lo][1] += c; }
-                        }
-                        cur_g = gi; ssum = 0.f; ssq = 0.f;
-                    }
-                    if (row_ok) {
-                        ssum += (o[j] + o[j + 1]) + (o[j + 2] + o[j + 3]);
-                        ssq += (o[j] * o[j] + o[j + 1] * o[j + 1]) + (o[j + 2] * o[j + 2] + o[j + 3] * o[j + 3]);
-                    }
-                }
-            }
-        }
-    }
-    if (STATS && cur_g >= 0) {
-        const float a = warp_sum(ssum), c = warp_sum(ssq);
-        if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] += a; sh->stats[ew][cur_g - g_lo][1] += c; }
-    }
-}
-
-// Persistent: CTA c processes tiles c, c + gridDim.x, ...  The TMA producer runs ahead across tile boundaries; the
-// accumulator is double-buffered in TMEM so the epilogue of tile i overlaps the main loop of tile i+1.
-template <int AMODE, bool RES, bool STATS, bool F16A, bool F16O>
-__global__ void __launch_bounds__(kThreads)
-tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
-                  const __grid_constant__ CUtensorMap mapW, const TapGemmArgs g, const int BN, const uint32_t idesc,
-                  const uint32_t tmem_cols, const int kStages, const int n_tiles, const int tiles_total) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int stage_bytes = kATileBytes + BN * 128;
-    TcShared* sh = reinterpret_cast<TcShared*>(smem + kStages * stage_bytes);
-    float* const sbias_f = reinterpret_cast<float*>(sh + 1);       // bias (or zeros), padded to whole 16-column chunks of the last tile
-    const uint32_t sbias = smem_u32(sbias_f);
-
-    using TO = typename std::conditional<F16O, __half, float>::type;
-    constexpr int kBKc = OperandKind<F16A>::kBK;
-    const aero_tapgemm_params& p = g.p;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nch1 = (p.C1 + kBKc - 1) / kBKc, nch2 = (p.C2 + kBKc - 1) / kBKc;
-    const bool mix = p.mode == AERO_TAPS_MIX;
-    const uint32_t acc_cols = tmem_cols >> 1;          // columns per accumulator buffer
-    // Epilogue organisation.  Wide tiles (tensor-bound): all eight warps drain one accumulator, two per TMEM lane quarter.
-    // Narrow tiles (HBM-bound layers, BN <= 64): the per-tile latency chain dominates, so the warps form two groups of
-    // four and each group drains every other tile on its own accumulator buffer -- two tiles in flight per CTA.
-    const bool grouped = BN <= g.grouped_bn;
-
-    for (int i = threadIdx.x; i < n_tiles * BN; i += kThreads) sbias_f[i] = (g.bias && i < g.p.N) ? g.bias[i] : 0.f;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&sh->acc_full[s], 1); mbar_init(&sh->acc_empty[s], grouped ? 16 * kEpiWarps : 32 * kEpiWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        for (int w = 0; w < kEpiWarps; ++w)
-            for (int i = 0; i < 8; ++i) { sh->stats[w][i][0] = 0.f; sh->stats[w][i][1] = 0.f; }
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sh->tmem_base)), "r"(tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = sh->tmem_base;
-
-    if (warp == 0) {
-        // ===================================================== TMA producer
-        if (lane == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA1) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
-            int stage = 0;
-            uint32_t phase = 0;
-            const uint32_t tx = (uint32_t)stage_bytes;
-            int ptl = 0;
-            for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x, ++ptl) {
-                const TileCoord c = tile_coord(g, tile, n_tiles, BN, nch1, nch2);
-                AERO_TRACE(0, ptl);
-                if (mix) {
-                    // A = activations [K rows][M contiguous].  tf32: four 32(m) x 32(k) boxes, f16: two 64(m) x 64(k) boxes
-                    // form one MN-major 128(m) x kBK(k) operand tile of 16 KB
-                    for (int kc = 0; kc < nch1; ++kc) {
-                        mbar_wait(&sh->empty[stage], phase ^ 1);
-                        uint8_t* sa = smem + stage * stage_bytes;
-                        mbar_expect_tx(&sh->full[stage], tx);
-                        constexpr int kBoxM = F16A ? 64 : 32;
-#pragma unroll
-                        for (int j = 0; j < 128 / kBoxM; ++j)
-                            tma_load_3d(sa + j * (kATileBytes / (128 / kBoxM)), &mapA1, &sh->full[stage], c.t0 + kBoxM * j, kc * kBKc, c.b);
-                        tma_load_3d(sa + kATileBytes, &mapW, &sh->full[stage], kc * kBKc, c.n0, 0);
-                        if (++stage == kStages) { stage = 0; phase ^= 1; }
-                    }
-                    continue;
-                }
-                for (int tap = 0; tap < g.ntaps; ++tap) {
-                    TapIter it;
-                    if (!tap_geometry(p, tap, c.fo, it)) continue;
-                    for (int src = 0; src < 2; ++src) {
-                        const int nch = src ? nch2 : nch1;
-                        const CUtensorMap* mA = src ? &mapA2 : &mapA1;
-                        const int kw0 = src ? p.C1 : 0;
-                        for (int kc = 0; kc < nch; ++kc) {
-                            mbar_wait(&sh->empty[stage], phase ^ 1);
-                            uint8_t* sa = smem + stage * stage_bytes;
-                            mbar_expect_tx(&sh->full[stage], tx);
-                            tma_load_4d(sa, mA, &sh->full[stage], kc * kBKc, c.t0 + it.dt, it.fi, c.b);
-                            tma_load_3d(sa + kATileBytes, &mapW, &sh->full[stage], kw0 + kc * kBKc, c.n0, it.slab);
-                            if (++stage == kStages) { stage = 0; phase ^= 1; }
-                        }
-                    }
-                }
-                AERO_TRACE(1, ptl);
-            }
-        }
-    } else if (warp == 1) {
-        // ===================================================== MMA issuer (the warp walks the pipeline, one elected lane issues)
-        {
-            int stage = 0;
-            uint32_t phase = 0;
-            int local = 0;
-            for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x, ++local) {
-                const TileCoord c = tile_coord(g, tile, n_tiles, BN, nch1, nch2);
-                const int buf = local & 1;
-                mbar_wait(&sh->acc_empty[buf], (uint32_t)(((local >> 1) & 1) ^ 1));     // epilogue has drained this buffer
-                tcgen05_fence_after();
-                AERO_TRACE(2, local);
-                const uint32_t tacc = tmem_base + (uint32_t)buf * acc_cols;
-                for (int i = 0; i < c.n_iters; ++i) {
-                    mbar_wait(&sh->full[stage], phase);
-                    tcgen05_fence_after();
-                    if (i == 0) AERO_TRACE(3, local);
-                    if (elect_one()) {
-                    const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-                    const uint64_t db = make_desc_sw128(sa + kATileBytes);
-                    if (mix && F16A) {
-                        // MN-major f16 A, plain SWIZZLE_128B (cute Layout_MN_SW128_Atom<half>): atoms of 64 elements along M
-                        // (128 B) x 8 rows along K = 1024 B.  A 64(m) x 64(k) TMA box is 8 K-atoms stacked (SBO = 1024 B); the two
-                        // boxes of a stage are the M atoms (LBO = 8192 B).  One UMMA (K = 16) consumes two K atoms = 2048 B.
-                        const uint64_t da = (uint64_t)((sa >> 4) & 0x3FFF) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-                                            ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma<F16A>(tacc, da + (uint64_t)(k * (2048 >> 4)), db + 2 * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    } else if (mix) {
-                        // MN-major tf32 A: the only legal layout is SWIZZLE_128B_BASE32B (cute Layout_MN_SW128_32B_Atom: 32 elements
-                        // along M x 4 rows along K = 512 B atoms, 32-byte chunks XOR-swizzled by row%4; TMA SWIZZLE_128B_ATOM_32B
-                        // writes exactly that).  A 32(m) x 32(k) TMA box is 8 K-atoms stacked (SBO = 512 B); the four boxes of a
-                        // stage are the M atoms (LBO = 4096 B).  One UMMA (K = 8) consumes two K atoms = 1024 B.
-                        const uint64_t da = (uint64_t)((sa >> 4) & 0x3FFF) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-                                            ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma<F16A>(tacc, da + (uint64_t)(k * (1024 >> 4)), db + 2 * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    } else {
-                        const uint64_t da = make_desc_sw128(sa);
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)             // one UMMA = 32 bytes along the swizzled row (K = 8 tf32 / 16 f16)
-                            umma<F16A>(tacc, da + 2 * k, db + 2 * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&sh->empty[stage]);
-                    }
-                    __syncwarp();
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-                if (elect_one()) umma_commit(&sh->acc_full[buf]);
-                __syncwarp();
-                AERO_TRACE(4, local);
-            }
-        }
-    } else {
-        // ===================================================== epilogue (warps 2..9)
-        const int q = warp & 3;                        // TMEM lane quarter this warp may access
-        const int ew = warp - 2;                       // epilogue warp index; ew >> 2 selects odd / even column chunks
-        const int m = q * 32 + lane;
-        const int Nout = p.glu ? p.N / 2 : p.N;
-        const int gw = (p.stats_mode == 1) ? Nout / p.groups : Nout;
-        const bool rnd = (p.flags & 1) && !F16O;
-        const int grp = ew >> 2;                       // grouped mode: which accumulator buffer / tile parity this warp serves
-        const int c_start = grouped ? 0 : grp * 16, c_step = grouped ? 16 : 32;
-        const int t_step = grouped ? 2 : 1;
-        const bool fast = !mix && g.vec_o && !g.colscale && (p.stats_mode == 0 || gw % 4 == 0);
-        int local = grouped ? grp : 0;
-        for (int64_t tile64 = (int64_t)blockIdx.x + (int64_t)local * gridDim.x; tile64 < tiles_total; tile64 += (int64_t)t_step * gridDim.x, local += t_step) {
-            const int tile = (int)tile64;
-            const TileCoord tc = tile_coord(g, tile, n_tiles, BN, nch1, nch2);
-            const int b = tc.b, fo = tc.fo, t0 = tc.t0, n0 = tc.n0, n_iters = tc.n_iters;
-            const int buf = local & 1;
-            const uint32_t tacc = tmem_base + (uint32_t)buf * acc_cols + ((uint32_t)(q * 32) << 16);
-            const int t = t0 + m;
-            const bool row_ok = t < p.T;
-            if (q == 0 && lane == 0) AERO_TRACE(5, local);
-            mbar_wait(&sh->acc_full[buf], (uint32_t)((local >> 1) & 1));
-            tcgen05_fence_after();
-            if (q == 0 && lane == 0) AERO_TRACE(6, local);
-            float sa = 1.f, sb = 0.f;
-            if (g.samp_affine) { sa = g.samp_affine[2 * b]; sb = g.samp_affine[2 * b + 1]; }
-            TO* op = static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + (int64_t)fo * p.o_sf + (int64_t)t * p.o_st;
-            const TO* rp = g.residual ? static_cast<const TO*>(g.residual) + (int64_t)b * p.r_sb + (int64_t)fo * p.r_sf + (int64_t)t * p.r_st : nullptr;
-            const float* csp = g.colscale ? g.colscale + (int64_t)b * p.cs_sb + (int64_t)t * p.cs_st : nullptr;
-            const float* adp = g.addend_fn ? g.addend_fn + (int64_t)fo * Nout : nullptr;
-            int cur_g = -1;
-            float ssum = 0.f, ssq = 0.f;
-            const int g_lo = (p.glu ? n0 >> 1 : n0) / gw;
-
-            if (mix) {
-                // transposed store: lane = pixel m (contiguous in memory), column = output row n
-                const float gate = (row_ok && g.colscale) ? g.colscale[(int64_t)b * p.cs_sb + t] : 1.f;
-                TO* ob = static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + t;
-                for (int c0 = c_start; c0 < BN; c0 += c_step) {
-                    uint32_t r[16];
-                    tmem_ld16(tacc + (uint32_t)c0, r);
-                    if (row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const int n = n0 + c0 + j;
-                            if (n < p.N) {
-                                float x = __uint_as_float(r[j]) * gate;
-                                if (rnd) x = round_tf32_rna(x);
-                                stf(ob + (int64_t)n * p.o_st, x);
-                            }
-                        }
-                    }
-                }
-            } else if (fast && (F16O ? (g.vec_o8 && (g.direct_f16 == 1 || (g.direct_f16 == 2 && AMODE == 3))) : g.direct_f32)) {
-                epilogue_direct<AMODE, RES, STATS, TO>(sh, g, tc, tacc, BN, q, ew, lane, Nout, gw, c_start, c_step, sbias);
-            } else if (fast) {
-                epilogue_fast_tile<AMODE, RES, STATS, TO>(sh, g, tc, tacc, BN, q, ew, lane, Nout, gw, c_start, c_step, sbias);
-            } else {
-                // generic (unaligned outputs / colscale) epilogue: lane = row, scattered stores; one warp per lane quarter
-                for (int c0 = 0; c0 < ((grouped || ew < 4) ? BN : 0); c0 += 16) {
-                    uint32_t r[16];
-                    if (n_iters > 0) {
-                        tmem_ld16(tacc + (uint32_t)c0, r);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) r[j] = 0u;
-                    }
-                    const int nb = n0 + c0;
-                    if (nb >= p.N) continue;                   // uniform: padded columns of the last tile
-                    float v[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int n = nb + j;
-                        float x = __uint_as_float(r[j]);
-                        if (row_ok && n < p.N) {
-                            x += sbias_f[n];
-                            if (csp) x *= csp[n];
-                            if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
-                            else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
-                        }
-                        v[j] = x;
-                    }
-                    float o[16];
-                    int no0, cnt;
-                    if (p.glu) {
-                        no0 = nb >> 1;
-                        cnt = 8;
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] = v[2 * j] * sigmoid_f(v[2 * j + 1]);
-                    } else {
-                        no0 = nb;
-                        cnt = 16;
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) o[j] = v[j];
-                    }
-                    // statistics bookkeeping is warp-uniform: groups depend on columns only
-#pragma unroll
-                    for (int sub = 0; sub < 2; ++sub) {
-                        if (sub * 8 >= cnt) break;
-                        const int ns = no0 + sub * 8;
-                        if (p.stats_mode != 0 && ns < Nout) {
-                            const int gi = ns / gw;
-                            if (gi != cur_g) {
-                                if (cur_g >= 0) {
-                                    const float a = warp_sum(ssum), c = warp_sum(ssq);
-                                    if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] = a; sh->stats[ew][cur_g - g_lo][1] = c; }
-                                }
-                                cur_g = gi; ssum = 0.f; ssq = 0.f;
-                            }
-                        }
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int jj = sub * 8 + j;
-                            const int nn = no0 + jj;
-                            if (row_ok && nn < Nout) {
-                                float x = o[jj];
-                                if (adp) x += adp[nn];
-                                if (rp) x += ldf(rp + nn);
-                                x = x * sa + sb;
-                                if (rnd) x = round_tf32_rna(x);
-                                x = stored(x, op);
-                                o[jj] = x;
-                                ssum += x;
-                                ssq += x * x;
-                            }
-                        }
-                    }
-                    if (row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (j < cnt && no0 + j < Nout) stf(op + no0 + j, o[j]);
-                    }
-                }
-                if (p.stats_mode != 0 && cur_g >= 0) {
-                    const float a = warp_sum(ssum), c = warp_sum(ssq);
-                    if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] = a; sh->stats[ew][cur_g - g_lo][1] = c; }
-                }
-            }
-            // accumulator buffer drained: hand it back to the MMA warp before the (cheap) statistics flush
-            tcgen05_fence_before();
-            mbar_arrive(&sh->acc_empty[buf]);
-            if (q == 0 && lane == 0) AERO_TRACE(7, local);
-            if (p.stats_mode != 0) {
-                // every warp publishes its own partial sums (fp64 atomics: the order across warps / CTAs only moves the last
-                // bits of a double): no CTA-wide barrier on the per-tile path
-                __syncwarp();
-                if (lane < 8) {
-                    const float a = sh->stats[ew][lane][0], c = sh->stats[ew][lane][1];
-                    const int gi = g_lo + lane;
-                    const int ngroups = (p.stats_mode == 1) ? p.groups : 1;
-                    if (gi < ngroups && (a != 0.f || c != 0.f)) {
-                        const int64_t slot = (p.stats_mode == 1) ? ((int64_t)b * p.groups + gi) : ((int64_t)b * p.F_out + fo);
-                        atomicAdd(&g.stats[2 * slot], (double)a);
-                        atomicAdd(&g.stats[2 * slot + 1], (double)c);
-                    }
-                    sh->stats[ew][lane][0] = 0.f;
-                    sh->stats[ew][lane][1] = 0.f;
-                }
-                __syncwarp();
-            }
-        }
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -725,7 +73,7 @@ int encode_map(CUtensorMap* out, const void* base, uint32_t rank, const uint64_t
     for (uint32_t i = 0; i + 1 < rank; ++i) gs[i] = strides_bytes[i];
     CUresult r = enc(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<void*>(base), gd, gs, bx, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     swizzle_mode == 1 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : swizzle_mode == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                     swizzle_mode == 2 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -740,21 +88,34 @@ int encode_map(CUtensorMap* out, const void* base, uint32_t rank, const uint64_t
     return AERO_OK;
 }
 
+// tile width: the narrowest built width (32, 64, 96, 128) that covers N in the fewest n-tiles
 static int pick_bn(int N) {
-    const int ntiles = (N + 255) / 256;
+    const int ntiles = (N + kMaxBN - 1) / kMaxBN;
     const int per = (N + ntiles - 1) / ntiles;
-    return (per + 15) & ~15;
+    return (per + 31) & ~31;
 }
 
-// precision 1: fp32 sources (kind::tf32); precision 2: FP16 sources (kind::f16).  TMA needs 16-byte global strides:
+// Shared memory of a CTA besides the pipeline stages: barriers / scratch, the bias of every column (padded to whole tiles) and the
+// accumulator staging tile.
+static int tc_fixed_smem(int N, int BN) { return (int)sizeof(TcShared) + cdiv(N, BN) * BN * 4 + kBM * (BN + 4) * 4 + 1024; }
+// Pipeline depth: the producer runs ahead across tiles, so depth is set by bytes in flight, not by the K length: as many stages as
+// fit.  Fewer than two cannot run (a stage is released only after the next one's wgmmas are issued).
+static int tc_stages(int N, int BN) {
+    if (N > (1 << 20)) return 0;
+    const int st = (227 * 1024 - tc_fixed_smem(N, BN)) / (kATileBytes + BN * 128);
+    return st > kMaxStages ? kMaxStages : st;
+}
+
+// precision 1: fp32 sources (tf32 wgmma); precision 2: FP16 sources (f16 wgmma).  TMA needs 16-byte global strides:
 // channel counts / strides in multiples of 4 fp32 or 8 halves.
 bool tapgemm_tc_eligible(const aero_tapgemm_params& p) {
     const bool f16 = (p.flags & AERO_TG_A_F16) != 0;
     const int q = f16 ? 8 : 4;
     if (p.mode == AERO_TAPS_MIX)
         return p.w_sb == 0 && p.C1 % q == 0 && p.C2 == 0 && p.a1_st % q == 0 && p.a1_sb % q == 0 && p.N >= 8 &&
-               p.stats_mode == 0 && !p.glu && p.F_out == 1 && p.F_in == 1;
+               p.stats_mode == 0 && !p.glu && p.F_out == 1 && p.F_in == 1 && tc_stages(p.N, pick_bn(p.N)) >= 2;
     if (p.w_sb != 0) return false;                                   // activations-as-weights (FTB frequency mix)
+    if (tc_stages(p.N, pick_bn(p.N)) < 2) return false;              // the bias of that many columns leaves no room for a pipeline
     if (p.N < 8) return false;                                       // thin outputs stay on the SIMT path
     const int K = p.C1 + p.C2;
     if (K < 8 || (p.C1 % q) || (p.C2 % q)) return false;
@@ -778,54 +139,16 @@ static int make_a_map(CUtensorMap* m, const void* base, int C, const aero_tapgem
     if (s3 <= 0) s3 = s2 * p.F_in;
     uint64_t strides[3] = {(uint64_t)s1 * esz, (uint64_t)s2 * esz, (uint64_t)s3 * esz};
     uint32_t box[4] = {(uint32_t)(128 / esz), (uint32_t)kBM, 1, 1};
-    return encode_map(m, base, 4, dims, strides, box, false, esz);
-}
-
-using KernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TapGemmArgs, int, uint32_t, uint32_t, int, int, int);
-
-// kernel variants: [operand kind][output type][AMODE][RES][STATS]; only the combinations the host code can produce are
-// instantiated for the FP16 kinds (statistics and fp32 outputs go together: GroupNorm inputs stay fp32)
-template <bool F16A, bool F16O>
-static KernelFn pick_kernel(int amode, bool res, bool stats) {
-#define AERO_TC_K(A, R, S) tapgemm_tc_kernel<A, R, S, F16A, F16O>
-    if constexpr (!F16A && !F16O) {
-        static const KernelFn table[4][2][2] = {
-            {{AERO_TC_K(0, false, false), AERO_TC_K(0, false, true)}, {AERO_TC_K(0, true, false), AERO_TC_K(0, true, true)}},
-            {{AERO_TC_K(1, false, false), AERO_TC_K(1, false, true)}, {AERO_TC_K(1, true, false), AERO_TC_K(1, true, true)}},
-            {{AERO_TC_K(2, false, false), AERO_TC_K(2, false, true)}, {AERO_TC_K(2, true, false), AERO_TC_K(2, true, true)}},
-            {{AERO_TC_K(3, false, false), AERO_TC_K(3, false, true)}, {AERO_TC_K(3, true, false), AERO_TC_K(3, true, true)}}};
-        return table[amode][res][stats];
-    } else if constexpr (F16O) {                   // FP16 outputs: statistics / residual only without activation
-        if (stats) return (amode == 0 && !res) ? AERO_TC_K(0, false, true) : nullptr;
-        if (res) return amode == 0 ? AERO_TC_K(0, true, false) : nullptr;
-        switch (amode) {
-            case 0: return AERO_TC_K(0, false, false);
-            case 1: return AERO_TC_K(1, false, false);
-            case 2: return AERO_TC_K(2, false, false);
-            default: return AERO_TC_K(3, false, false);
-        }
-    } else {
-        // FP16 operands, fp32 outputs: pre-normalisation outputs (with statistics), LSTM gate inputs, attention q/k/v, FTB gate
-        if (res) return nullptr;
-        if (stats) return amode == 0 ? AERO_TC_K(0, false, true) : nullptr;
-        switch (amode) {
-            case 0: return AERO_TC_K(0, false, false);
-            case 1: return AERO_TC_K(1, false, false);
-            case 2: return AERO_TC_K(2, false, false);
-            default: return AERO_TC_K(3, false, false);      // fp32 GLU output: the last decoder layer (feeds the exact-fp32 conv-T)
-        }
-    }
-#undef AERO_TC_K
+    return encode_map(m, base, 4, dims, strides, box, 0, esz);
 }
 
 // tuning knobs (tools/kprof.py), read from the environment ONCE when the library first launches this kernel: the launch
 // path itself never calls getenv.  -1 = not set.
 struct TcKnobs {
-    int direct_f32 = -1, direct_f16 = -1, grouped_bn = -1, stages = -1, per_sm = -1;
+    int direct_f32 = -1, direct_f16 = -1, stages = -1;
     TcKnobs() {
         auto rd = [](const char* name, int& v) { if (const char* e = getenv(name)) v = atoi(e); };
-        rd("AERO_TC_DIRECT_F32", direct_f32); rd("AERO_TC_DIRECT_F16", direct_f16); rd("AERO_TC_GROUPED_BN", grouped_bn);
-        rd("AERO_TC_STAGES", stages); rd("AERO_TC_PER_SM", per_sm);
+        rd("AERO_TC_DIRECT_F32", direct_f32); rd("AERO_TC_DIRECT_F16", direct_f16); rd("AERO_TC_STAGES", stages);
     }
 };
 static const TcKnobs& knobs() { static const TcKnobs k; return k; }
@@ -847,7 +170,7 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
         uint64_t dims[3] = {(uint64_t)p.T, (uint64_t)p.C1, (uint64_t)p.B};
         uint64_t strides[2] = {(uint64_t)p.a1_st * esz, (uint64_t)(p.a1_sb > 0 ? p.a1_sb : (int64_t)p.a1_st * p.C1) * esz};
         uint32_t box[3] = {(uint32_t)(f16a ? 64 : 32), (uint32_t)kBKc, 1};
-        if ((rc = encode_map(&mA1, g.a1, 3, dims, strides, box, !f16a, esz)) != AERO_OK) return rc;
+        if ((rc = encode_map(&mA1, g.a1, 3, dims, strides, box, 0, esz)) != AERO_OK) return rc;
     } else if (p.C1) { if ((rc = make_a_map(&mA1, g.a1, p.C1, p, p.a1_sb, p.a1_sf, p.a1_st, esz)) != AERO_OK) return rc; }
     if (p.C2) { if ((rc = make_a_map(&mA2, g.a2, p.C2, p, p.a2_sb, p.a2_sf, p.a2_st, esz)) != AERO_OK) return rc; }
     if (!p.C1) mA1 = mA2;
@@ -859,15 +182,13 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
         uint64_t dims[3] = {(uint64_t)K, npad, (uint64_t)nslab};
         uint64_t strides[2] = {kp * esz, kp * npad * esz};
         uint32_t box[3] = {(uint32_t)kBKc, (uint32_t)BN, 1};
-        if ((rc = encode_map(&mW, g.w, 3, dims, strides, box, false, esz)) != AERO_OK) return rc;
+        if ((rc = encode_map(&mW, g.w, 3, dims, strides, box, 0, esz)) != AERO_OK) return rc;
     }
     g.tiles_t = cdiv(p.T, kBM);
-    g.grouped_bn = 128;
     g.direct_f32 = 0;
-    g.direct_f16 = 2;       // measured: the direct form wins for GLU outputs (one 16-byte store per lane), the transpose otherwise
+    g.direct_f16 = 2;       // GLU outputs take the direct form (one 16-byte store per lane), the others the transpose
     if (kn.direct_f32 >= 0) g.direct_f32 = kn.direct_f32;
     if (kn.direct_f16 >= 0) g.direct_f16 = kn.direct_f16;
-    if (kn.grouped_bn >= 0) g.grouped_bn = kn.grouped_bn;
     const int64_t tiles = (int64_t)p.B * p.F_out * g.tiles_t;
     if (tiles > 2147483647LL) { set_error("aero_tapgemm_fwd: too many tiles"); return AERO_ERR_INVALID; }
     {
@@ -880,44 +201,29 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
             g.dv_shr[i] = 31 + s;
         }
     }
-    uint32_t tmem_cols = 32;                       // two accumulator buffers (double-buffered epilogue)
-    while ((int)tmem_cols < BN) tmem_cols <<= 1;
-    tmem_cols <<= 1;
-    // cute::UMMA::InstrDescriptor: D=F32 (1<<4), A/B format at [7,10)/[10,13) (F16 = 0, TF32 = 2), K-major both,
-    // N>>3 at [17,23), M>>4 at [24,29)
-    const uint32_t fmt = f16a ? 0u : 2u;
-    const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24) |
-                           (mix ? (1u << 15) : 0u);                 // bit 15: A is MN-major
-    const int nch = (p.C1 + kBKc - 1) / kBKc + (p.C2 + kBKc - 1) / kBKc;
-    const int max_iters = nch * ((p.mode == AERO_TAPS_CONVT) ? p.kf / p.stride_f : p.kf * p.kt);
     const int stage_bytes = kATileBytes + BN * 128;
-    // pipeline depth: the producer runs ahead across tiles, so depth is set by bytes in flight, not by the K length.
-    // Long K loops get as many stages as fit; short, HBM-bound layers keep ~64 KB in flight and leave room for 2-3 CTAs/SM.
-    const int bias_bytes = cdiv(p.N, BN) * BN * 4;
-    const int fixed = (int)sizeof(TcShared) + bias_bytes + 1024;
-    int kStages;
-    if (max_iters >= (f16a ? 12 : 24)) {
-        kStages = (227 * 1024 - fixed) / stage_bytes;
-    } else {
-        kStages = (96 * 1024) / stage_bytes;
+    const int fixed = tc_fixed_smem(p.N, BN);
+    int kStages = tc_stages(p.N, BN);
+    if (kStages < 2) {
+        set_error("aero_tapgemm_fwd(wgmma): N = %d leaves no shared memory for the pipeline", p.N);
+        return AERO_ERR_UNSUPPORTED;
     }
-    if (kn.stages >= 0) kStages = kn.stages;
-    if (kStages > kMaxStages) kStages = kMaxStages;
-    if (kStages < 2) kStages = 2;
-    while (kStages > 2 && (size_t)kStages * stage_bytes + fixed > 227 * 1024) --kStages;
+    if (kn.stages >= 2 && kn.stages < kStages) kStages = kn.stages;
     const size_t smem = (size_t)kStages * stage_bytes + fixed;
     const int amode = p.glu ? 3 : p.act;                 // the engine never combines GLU with an activation
-    if (p.glu && p.act != AERO_ACT_NONE) { set_error("aero_tapgemm_fwd(tcgen05): GLU with an activation is not supported"); return AERO_ERR_UNSUPPORTED; }
+    if (p.glu && p.act != AERO_ACT_NONE) { set_error("aero_tapgemm_fwd(wgmma): GLU with an activation is not supported"); return AERO_ERR_UNSUPPORTED; }
     const bool res = g.residual != nullptr, stats = p.stats_mode != 0;
-    const KernelFn kern = f16a ? (f16o ? pick_kernel<true, true>(amode, res, stats) : pick_kernel<true, false>(amode, res, stats))
-                               : (f16o ? pick_kernel<false, true>(amode, res, stats) : pick_kernel<false, false>(amode, res, stats));
+    const KernelFn kern = BN == 32 ? tapgemm_tc_kernels_bn32(f16a, f16o, amode, res, stats)
+                        : BN == 64 ? tapgemm_tc_kernels_bn64(f16a, f16o, amode, res, stats)
+                        : BN == 96 ? tapgemm_tc_kernels_bn96(f16a, f16o, amode, res, stats)
+                                   : tapgemm_tc_kernels_bn128(f16a, f16o, amode, res, stats);
     if (!kern) {
-        set_error("aero_tapgemm_fwd(tcgen05): epilogue (act %d, residual %d, stats %d) is not built for operands %s / outputs %s",
+        set_error("aero_tapgemm_fwd(wgmma): epilogue (act %d, residual %d, stats %d) is not built for operands %s / outputs %s",
                   amode, (int)res, (int)stats, f16a ? "f16" : "tf32", f16o ? "f16" : "f32");
         return AERO_ERR_UNSUPPORTED;
     }
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    // persistent grid: as many CTAs as can be co-resident (shared memory and TMEM columns), never more than tiles
+    // persistent grid: one CTA per SM (the pipeline and the staging tile take the shared memory), never more than tiles
     static int num_sms = 0;
     if (num_sms == 0) {
         int dev = 0;
@@ -927,16 +233,11 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
     const int n_tiles = cdiv(p.N, BN);
     const int64_t tiles_total = tiles * n_tiles;
     if (tiles_total > 2147483647LL) { set_error("aero_tapgemm_fwd: too many tiles"); return AERO_ERR_INVALID; }
-    int per_sm = (int)((227 * 1024) / (smem + 1024));
-    if (per_sm > (int)(512 / tmem_cols)) per_sm = (int)(512 / tmem_cols);
-    if (per_sm > 2) per_sm = 2;                      // 320 threads x ~96 registers: two CTAs per SM
-    if (kn.per_sm >= 0 && kn.per_sm < per_sm) per_sm = kn.per_sm;
-    if (per_sm < 1) per_sm = 1;
-    const int64_t want = (int64_t)num_sms * per_sm;
+    const int64_t want = num_sms;
     g.last_tile = (int)tiles_total - 1;
     dim3 grid((unsigned)(tiles_total < want ? tiles_total : want));
-    kern<<<grid, kThreads, smem, st>>>(mA1, mA2, mW, g, BN, idesc, tmem_cols, kStages, n_tiles, (int)tiles_total);
-    return check_launch("aero_tapgemm_fwd(tcgen05)");
+    kern<<<grid, kThreads, smem, st>>>(mA1, mA2, mW, g, kStages, n_tiles, (int)tiles_total);
+    return check_launch("aero_tapgemm_fwd(wgmma)");
 }
 
 }  // namespace aero

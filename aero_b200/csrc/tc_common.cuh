@@ -1,13 +1,13 @@
-// tcgen05 / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_100a).
+// TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a); the wgmma wrappers are in wgmma.cuh.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace aero {
 
 // host: cached cuTensorMapEncodeTiled (fp32, SWIZZLE_128B, zero OOB fill); implemented in tapgemm_tc.cu
-// swizzle_mode: 0 = CU_TENSOR_MAP_SWIZZLE_128B; 1 = SWIZZLE_128B_ATOM_32B (pairs with UMMA SWIZZLE_128B_BASE32B, the only layout
-// for MN-major tf32); 2 = SWIZZLE_64B (64-byte operand rows)
+// swizzle_mode: 0 = CU_TENSOR_MAP_SWIZZLE_128B; 2 = SWIZZLE_64B (64-byte operand rows)
 int encode_map(CUtensorMap* out, const void* base, uint32_t rank, const uint64_t* dims, const uint64_t* strides_bytes,
                const uint32_t* box, int swizzle_mode = 0, int elem_bytes = 4);
 
@@ -30,13 +30,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug must abort the kernel, not hang the GPU.
+// Bounded wait: a protocol bug must abort the kernel, not hang the GPU.  The abort is a bare trap: a printf here would be a
+// function call inside the loops that keep wgmma groups in flight, and ptxas serialises every wgmma across a call.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin) {
-        if (spin > (1u << 24)) {
-            printf("aero tapgemm_tc: mbarrier timeout (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-            __trap();
-        }
+        if (spin > (1u << 24)) asm volatile("trap;");
     }
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
@@ -49,73 +47,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-// One lane of a converged warp.  tcgen05 issue code guarded by this (rather than by `lane == 0`) lets the compiler emit the
-// MMAs back to back instead of wrapping each one in its own election loop.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, 0xffffffff;\n\t"
-        "@px mov.s32 %0, 1;\n\t}"
-        : "+r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-template <bool F16>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    if (F16) umma_f16(tmem_d, desc_a, desc_b, idesc, accumulate);
-    else umma_tf32(tmem_d, desc_a, desc_b, idesc, accumulate);
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14),
-// LBO>>4 [16,30) (=1, unused for swizzled K-major), SBO>>4 [32,46) (8 rows x 128 B = 1024), version 1 [46,48),
-// layout type SWIZZLE_128B = 2 [61,64).
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
         : "memory");
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
@@ -135,6 +66,16 @@ __device__ __forceinline__ void sts128(uint32_t saddr, float4 v) {
 __device__ __forceinline__ void sts64(uint32_t saddr, float a, float b) {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(a), "f"(b) : "memory");
 }
+// 16 consecutive fp32 of an accumulator row staged in shared memory (16-byte aligned)
+__device__ __forceinline__ void acc_ld16(uint32_t saddr, uint32_t (&r)[16]) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float4 v = lds128(saddr + 16u * j);
+        r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y); r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
+    }
+}
+// barrier over the 128 threads of one warpgroup (id 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }

@@ -292,7 +292,7 @@ __global__ void __launch_bounds__(kWsThreads) wgrad_thin_n_kernel(const WgradArg
 }
 
 // ------------------------------------------------------------------------------------------------------------ weight repack
-// [taps][K][ldn] (N contiguous: the SIMT tap-GEMM layout) -> [taps][ldn][K] (K contiguous: the tcgen05 layout), rounded to TF32
+// [taps][K][ldn] (N contiguous: the SIMT tap-GEMM layout) -> [taps][ldn][K] (K contiguous: the wgmma layout), rounded to TF32
 // (round-to-nearest, ties away: cvt.rna) -- the training step repacks every weight it uses, every step, so this is one launch instead
 // of a transpose, an add and a mask.
 __global__ void __launch_bounds__(256) pack_kmajor_tf32_kernel(const float* __restrict__ w, float* __restrict__ out, float* __restrict__ out_lo,
@@ -877,7 +877,7 @@ extern "C" int aero_tapgemm_wgrad(const float* a1, const float* a2, const float*
     g.dw_sn = dw_sn; g.dw_sk = dw_sk; g.dw_ss = dw_ss;
     const int K = p->C1 + p->C2;
     g.tiles_t = cdiv(p->T, kWgP);
-    // (the 8 x 8 variant, TN = 128, measured no faster on B200 -- 138.9 vs 136.7 ms per generator step -- so the narrow one serves all;
+    // (the 8 x 8 variant, TN = 128, is kept for experiments; it has not been compared on H100, so the narrow one serves all;
     //  AERO_WGRAD_WIDE=1 selects it for experiments)
     static const bool wide = getenv("AERO_WGRAD_WIDE") != nullptr;
     const int TN = (wide && p->N >= 128) ? 128 : 64;
@@ -892,7 +892,7 @@ extern "C" int aero_tapgemm_wgrad(const float* a1, const float* a2, const float*
     if ((int64_t)nslab * K * p->N <= kWsPer * kWsThreads && (int64_t)p->B * p->F_out * p->T >= 4096) {
         // few weights, many pixels: one thread per weight
         const int64_t n_rows = (int64_t)p->B * p->F_out;
-        int n_seg = (int)cdiv((int64_t)148 * 8, n_rows);
+        int n_seg = (int)cdiv((int64_t)132 * 8, n_rows);
         if (n_seg > cdiv(p->T, 32)) n_seg = cdiv(p->T, 32);
         if (n_seg < 1) n_seg = 1;
         const int seg_len = cdiv(p->T, n_seg);
@@ -907,7 +907,7 @@ extern "C" int aero_tapgemm_wgrad(const float* a1, const float* a2, const float*
     }
     // enough CTAs to fill the GPU a few times over, never more than chunks
     int64_t tiles = (int64_t)g.k_tiles * g.n_tiles * nslab;
-    int64_t splits = (148 * 6 + tiles - 1) / tiles;
+    int64_t splits = (132 * 6 + tiles - 1) / tiles;
     if (splits > n_chunks) splits = n_chunks;
     if (splits > 65535) splits = 65535;
     if (splits < 1) splits = 1;
@@ -931,7 +931,7 @@ extern "C" int aero_split_tf32(const float* x, float* hi, float* lo, int64_t n, 
     AERO_REQUIRE(x && hi && lo && n >= 1, "aero_split_tf32: bad argument");
     AERO_REQUIRE((((uintptr_t)x | (uintptr_t)hi | (uintptr_t)lo) & 15) == 0, "aero_split_tf32: 16-byte aligned buffers");
     int64_t blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     split_tf32_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, hi, lo, n);
     return check_launch("aero_split_tf32");
@@ -951,7 +951,7 @@ extern "C" int aero_colsum(const float* x, const float* z, void* out1, void* out
         ((((uintptr_t)x) | ((uintptr_t)z)) & 15) == 0) {
         const int xt = cdiv(N, 128);
         int64_t ys = (rows + 8 * 16 - 1) / (8 * 16);                   // at least 16 rows per thread
-        const int64_t cap4 = (int64_t)148 * 8 / ((int64_t)xt * n_seg) + 1;
+        const int64_t cap4 = (int64_t)132 * 8 / ((int64_t)xt * n_seg) + 1;
         if (ys > cap4) ys = cap4;
         if (ys < 1) ys = 1;
         if (ys > 65535) ys = 65535;
@@ -965,7 +965,7 @@ extern "C" int aero_colsum(const float* x, const float* z, void* out1, void* out
         return check_launch("aero_colsum");
     }
     int64_t ysplit = (rows + 8 * 64 - 1) / (8 * 64);
-    const int64_t cap = (int64_t)148 * 16 / (cdiv(N, 32) * (int64_t)n_seg) + 1;
+    const int64_t cap = (int64_t)132 * 16 / (cdiv(N, 32) * (int64_t)n_seg) + 1;
     if (ysplit > cap) ysplit = cap;
     if (ysplit < 1) ysplit = 1;
     if (ysplit > 65535) ysplit = 65535;
@@ -984,7 +984,7 @@ extern "C" int aero_gram(const float* P, const float* Q, const float* gate, floa
     using namespace aero;
     AERO_REQUIRE(P && Q && out && B >= 1 && F >= 1 && M >= 1, "aero_gram: bad argument");
     const int tiles = cdiv(F, 64);
-    int chunks = (148 * 4) / (tiles * tiles * B) + 1;
+    int chunks = (132 * 4) / (tiles * tiles * B) + 1;
     const int64_t max_chunks = (M + 31) / 32;
     if (chunks > max_chunks) chunks = (int)max_chunks;
     AERO_REQUIRE((int64_t)B * chunks <= 65535, "aero_gram: too many z blocks");
@@ -998,7 +998,7 @@ extern "C" int aero_bcast_add(float* x, const float* addend, int32_t B, int32_t 
     AERO_REQUIRE(x && addend && B >= 1 && F >= 1 && T >= 1 && C >= 4 && C % 4 == 0, "aero_bcast_add: bad argument");
     const int64_t total4 = (int64_t)B * F * T * (C / 4);
     int64_t blocks = (total4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     bcast_add_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(x, addend, total4, F, T, C);
     return check_launch("aero_bcast_add");
 }
@@ -1018,7 +1018,7 @@ extern "C" int aero_add(float* dst, const float* src, int64_t n, float alpha, ae
     AERO_REQUIRE(dst && src && n >= 0 && ((((uintptr_t)dst | (uintptr_t)src) & 15) == 0), "aero_add: bad argument");
     if (n == 0) return AERO_OK;
     int64_t blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     add_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(dst, src, n, alpha);
     return check_launch("aero_add");
@@ -1029,7 +1029,7 @@ extern "C" int aero_add_f64(float* dst, const double* src, int64_t n, aero_strea
     AERO_REQUIRE(dst && src && n >= 0, "aero_add_f64: bad argument");
     if (n == 0) return AERO_OK;
     int64_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     add_f64_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(dst, src, n);
     return check_launch("aero_add_f64");
 }

@@ -485,7 +485,7 @@ extern "C" int aero_gconv1d_wgrad(const float* x, const float* dy, float* dw, in
         const size_t smem4 = sizeof(float) * ((size_t)kG4Co * kG4Dy + (size_t)nch * kG4Xw);
         cudaFuncSetAttribute(gconv41_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4);
         const int n_tiles4 = B * cdiv(Tout, kG4T);
-        int chunks4 = (148 * 4) / (Cout / kG4Co) + 1;
+        int chunks4 = (132 * 4) / (Cout / kG4Co) + 1;
         if (chunks4 > n_tiles4) chunks4 = n_tiles4;
         if (chunks4 > 65535) chunks4 = 65535;
         dim3 grid4(Cout / kG4Co, chunks4);
@@ -497,7 +497,7 @@ extern "C" int aero_gconv1d_wgrad(const float* x, const float* dy, float* dw, in
     const size_t smem = gconv_smem(p, 0);
     cudaFuncSetAttribute(gconv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const int64_t n_tiles = (int64_t)B * cdiv(Tout, kGcT);
-    int chunks = (148 * 4) / cdiv(Cout, kGcCo) + 1;
+    int chunks = (132 * 4) / cdiv(Cout, kGcCo) + 1;
     if (chunks > n_tiles) chunks = (int)n_tiles;
     if (chunks > 65535) chunks = 65535;
     dim3 grid(cdiv(Cout, kGcCo), chunks);

@@ -324,7 +324,7 @@ extern "C" int aero_lstm_fold(const float* dgin_w, float* dgin, int32_t rows, in
     AERO_REQUIRE(n_win == 1 || win_stride >= 1, "aero_lstm_fold: win_stride");
     const int64_t total = (int64_t)rows * T * (C / 4);
     int64_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     lstm_fold_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(dgin_w, dgin, rows, T, n_win, steps, win_stride, C);
     return check_launch("aero_lstm_fold");
 }

@@ -1,18 +1,19 @@
-// Weight gradient of the tap-GEMM on the tensor cores (sm_100a, kind::tf32): the training-side twin of tapgemm_tc.cu.
+// Weight gradient of the tap-GEMM on the tensor cores (sm_90a, TF32): the training-side twin of tapgemm_tc.cu.
 //
 //   dW[slab][k][n] += sum over output pixels (b, fo, t) of  A(b, fi, t + dt, k) * dY(b, fo, t, n)
 //
 // is, per slab, a GEMM whose reduction axis is the pixel axis -- the axis that is NOT contiguous in the channels-last tensors.  Both
-// operands are therefore MN-major for tcgen05 (cute Layout_MN_SW128_32B_Atom, the only MN-major form of tf32): a TMA box of
-// 32 channels x 32 consecutive frames of one (b, f) row, written with SWIZZLE_128B_ATOM_32B, is 8 K-atoms (4 frames x 128 B) of one
-// 32-channel M atom.  No transposition pass, no im2col: the tap shift is the box coordinate, borders and tails are TMA zero fill.
+// operands are therefore MN-major.  wgmma reads tf32 operands from shared memory K-major only, so this kernel keeps the TMA /
+// mbarrier pipeline and feeds mma.sync.m16n8k8 (tf32) from registers: the fragment loads do the transposition.  A TMA box is
+// 32 channels x 32 consecutive frames of one (b, f) row, SWIZZLE_128B (row = frame, 128 B of channels, 16-byte unit ^ (frame % 8)):
+// no transposition pass, no im2col: the tap shift is the box coordinate, borders and tails are TMA zero fill.
 //
-//   D (TMEM)  : 128 lanes = 128 output channels n, BN <= 256 fp32 columns = input channels k (32-channel boxes taken from the
-//               concatenation of the two source tensors of a skip connection; a box never straddles them)
-//   A (smem)  : dY tile  [32 frames][128 n]  = 4 boxes, 16 KB
-//   B (smem)  : act tile [32 frames][BN k]   = BN/32 boxes
-// One CTA owns one (slab, n-tile, k-tile) and a strided subset of the 32-frame chunks (split-K over pixels); warp 0 = TMA producer,
-// warp 1 = MMA issue, warps 2..5 = epilogue: TMEM -> red.global.add.f32 into dW in the parameter's own layout (dW is zeroed by the
+//   D (registers) : 128 output channels n (16 per warp) x BN <= 128 input channels k (32-channel boxes taken from the
+//                   concatenation of the two source tensors of a skip connection; a box never straddles them)
+//   A (smem)      : dY tile  [32 frames][128 n]  = 4 boxes, 16 KB
+//   B (smem)      : act tile [32 frames][BN k]   = BN/32 boxes
+// One CTA owns one (slab, n-tile, k-tile) and a strided subset of the 32-frame chunks (split-K over pixels); warp 8 = TMA producer,
+// warps 0..7 = MMA, then red.global.add.f32 into dW in the parameter's own layout (dW is zeroed by the
 // caller; same contract as the SIMT kernel in train.cu).  The tensor core reads fp32 bit patterns and ignores the low 13 mantissa
 // bits (truncation, as cuDNN's TF32 convolutions do): this is the precision-1 training mode, not the parity mode.
 #include <cuda.h>
@@ -21,17 +22,16 @@
 
 namespace aero {
 
-constexpr int kWtThreads = 192;
+constexpr int kWtMmaWarps = 8;
+constexpr int kWtThreads = 32 * kWtMmaWarps + 32;
+constexpr int kWtMaxBoxes = 4;          // 32-channel boxes per k-tile: 16 accumulators per box and thread
 constexpr int kWtMaxStages = 8;
-constexpr int kWtChunk = 32;              // frames per pipeline stage (= 4 UMMAs of K = 8)
+constexpr int kWtChunk = 32;              // frames per pipeline stage (= 4 MMA steps of K = 8)
 constexpr int kWtATile = 128 * 128;       // 4 boxes x 4 KB
 
 struct WgradTcShared {
     uint64_t full[kWtMaxStages];
     uint64_t empty[kWtMaxStages];
-    uint64_t acc_full;
-    uint32_t tmem_base;
-    int has_acc;
 };
 
 struct WgradTcArgs {
@@ -40,12 +40,10 @@ struct WgradTcArgs {
     int64_t dw_sn, dw_sk, dw_ss;
     int tiles_t, n_tiles, k_tiles, nb1, nb, bpt, BN, splits, stages;   // nb1 / nb: 32-channel boxes of source 1 / of both; bpt: boxes per k-tile
     int d_tt, d_fo, d_b;                                               // `splits` chunks ahead, as (frame-chunk, row, batch) carries
-    uint32_t idesc, tmem_cols;
 };
 
 // Walks the 32-frame chunks split, split + splits, ... of the (b, fo, frame-chunk) space with carries only: the walkers are single
-// threads (TMA producer, MMA issuer) whose every instruction is on the critical path -- a 64-bit division per chunk costs more than the
-// chunk's four UMMAs.
+// on the critical path of the pipeline: no division per chunk.
 struct WtWalker {
     int b, fo, tt;
     __device__ __forceinline__ void init(const WgradTcArgs& g, int split) {
@@ -78,7 +76,14 @@ struct WtWalker {
     }
 };
 
-__global__ void __launch_bounds__(kWtThreads)
+// element (frame f, channel ch) of a 32 x 32 SWIZZLE_128B box at shared address `box`
+__device__ __forceinline__ uint32_t wt_lds(uint32_t box, int f, int ch) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(box + (uint32_t)(f * 128 + (((ch >> 2) ^ (f & 7)) << 4) + ((ch & 3) << 2))));
+    return v;
+}
+
+__global__ void __launch_bounds__(kWtThreads, 2)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant__ CUtensorMap mapA2,
                 const __grid_constant__ CUtensorMap mapDy, const WgradTcArgs g) {
     extern __shared__ uint8_t smem_raw[];
@@ -104,21 +109,12 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant
     }
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < g.stages; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], 1); }
-        mbar_init(&sh->acc_full, 1);
-        sh->has_acc = 1;
+        for (int s = 0; s < g.stages; ++s) { mbar_init(&sh->full[s], 1); mbar_init(&sh->empty[s], kWtMmaWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sh->tmem_base)), "r"(g.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = sh->tmem_base;
 
-    if (warp == 0) {
+    if (warp == kWtMmaWarps) {
         // ===================================================== TMA producer
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA1) : "memory");
@@ -144,8 +140,16 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant
                 if (++stage == g.stages) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===================================================== MMA issuer
+    } else {
+        // ===================================================== MMA warps: warp w owns output channels n0 + 16 w .. + 15, all boxes
+        const int gq = lane >> 2, c = lane & 3;
+        float acc[kWtMaxBoxes][4][4];
+#pragma unroll
+        for (int j = 0; j < kWtMaxBoxes; ++j)
+#pragma unroll
+            for (int t = 0; t < 4; ++t)
+#pragma unroll
+                for (int u = 0; u < 4; ++u) acc[j][t][u] = 0.f;
         int stage = 0;
         uint32_t phase = 0;
         int iters = 0;
@@ -154,64 +158,53 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_constant
             int fi_unused;
             if (!w.input_row(p, jf, r, tapi, fi_unused)) continue;         // same enumeration as the producer
             mbar_wait(&sh->full[stage], phase);
-            tcgen05_fence_after();
-            if (elect_one()) {
-                const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-                // MN-major tf32 operands (see tapgemm_tc.cu, the frequency-mix mode): LBO = 4096 B between 32-channel atoms (boxes),
-                // SBO = 512 B between 4-frame K atoms, layout SWIZZLE_128B_BASE32B; one UMMA (K = 8 frames) = two K atoms = 1024 B
-                const uint64_t da = (uint64_t)((sa >> 4) & 0x3FFF) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-                                    ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
-                const uint32_t sb = sa + kWtATile;
-                const uint64_t db = (uint64_t)((sb >> 4) & 0x3FFF) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-                                    ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
+            const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+            const uint32_t abox = sa + (uint32_t)(warp >> 1) * 4096u;
+            const int ach = (warp & 1) * 16 + gq;
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    umma_tf32(tmem_base, da + (uint64_t)(k * (1024 >> 4)), db + (uint64_t)(k * (1024 >> 4)), g.idesc, (iters > 0 || k > 0) ? 1u : 0u);
-                umma_commit(&sh->empty[stage]);
+            for (int kk = 0; kk < kWtChunk / 8; ++kk) {
+                const int f = 8 * kk + c;
+                const uint32_t a0 = wt_lds(abox, f, ach), a1 = wt_lds(abox, f, ach + 8), a2 = wt_lds(abox, f + 4, ach), a3 = wt_lds(abox, f + 4, ach + 8);
+#pragma unroll
+                for (int j = 0; j < kWtMaxBoxes; ++j) {
+                    if (j < nbox) {
+                        const uint32_t bbox = sa + kWtATile + (uint32_t)j * 4096u;
+#pragma unroll
+                        for (int t = 0; t < 4; ++t) {
+                            const uint32_t b0 = wt_lds(bbox, f, 8 * t + gq), b1 = wt_lds(bbox, f + 4, 8 * t + gq);
+                            asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                                         : "+f"(acc[j][t][0]), "+f"(acc[j][t][1]), "+f"(acc[j][t][2]), "+f"(acc[j][t][3])
+                                         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+                        }
+                    }
+                }
             }
             __syncwarp();
+            if (lane == 0) mbar_arrive(&sh->empty[stage]);
             ++iters;
             if (++stage == g.stages) { stage = 0; phase ^= 1; }
         }
-        if (elect_one()) {
-            if (iters > 0) {
-                umma_commit(&sh->acc_full);
-            } else {
-                sh->has_acc = 0;
-                mbar_arrive(&sh->acc_full);
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================================================== epilogue (warps 2..5): TMEM -> atomics on dW
-        const int q = warp & 3;                                // TMEM lane quarter of this warp
-        const int n = n0 + q * 32 + lane;
-        mbar_wait(&sh->acc_full, 0);
-        tcgen05_fence_after();
-        if (sh->has_acc) {
-            const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16);
-            float* dst_n = g.dw + (int64_t)n * g.dw_sn + (int64_t)slab * g.dw_ss;
-            for (int j = 0; j < nbox; ++j) {                   // one 32-column block per box
-                const int gb = box0 + j;
-                const bool s2 = gb >= g.nb1;
-                const int ch0 = 32 * (s2 ? gb - g.nb1 : gb);
-                const int cnt = min(32, (s2 ? p.C2 : p.C1) - ch0);
-                const int kbase = (s2 ? p.C1 : 0) + ch0;
-                uint32_t v[32];
-                tmem_ld32(tacc + (uint32_t)(32 * j), v);
-                if (n < p.N) {
+        // ===================================================== epilogue: atomics on dW
+        if (iters > 0) {
 #pragma unroll
-                    for (int u = 0; u < 32; ++u)
-                        if (u < cnt) atomicAdd(dst_n + (int64_t)(kbase + u) * g.dw_sk, __uint_as_float(v[u]));
+            for (int j = 0; j < kWtMaxBoxes; ++j) {
+                if (j < nbox) {
+                    const int gb = box0 + j;
+                    const bool s2 = gb >= g.nb1;
+                    const int ch0 = 32 * (s2 ? gb - g.nb1 : gb);
+                    const int cnt = min(32, (s2 ? p.C2 : p.C1) - ch0);
+                    const int kbase = (s2 ? p.C1 : 0) + ch0;
+#pragma unroll
+                    for (int t = 0; t < 4; ++t)
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) {
+                            const int n = n0 + 16 * warp + gq + (u >> 1) * 8, kc = 8 * t + 2 * c + (u & 1);
+                            if (n < p.N && kc < cnt)
+                                atomicAdd(g.dw + (int64_t)n * g.dw_sn + (int64_t)slab * g.dw_ss + (int64_t)(kbase + kc) * g.dw_sk, acc[j][t][u]);
+                        }
                 }
             }
         }
-        tcgen05_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(g.tmem_cols) : "memory");
     }
 }
 
@@ -222,7 +215,7 @@ static int wt_map(CUtensorMap* m, const void* base, int C, int T, int F, int B, 
     if (s3 <= 0) s3 = s2 * F;
     uint64_t strides[3] = {(uint64_t)s1 * 4, (uint64_t)s2 * 4, (uint64_t)s3 * 4};
     uint32_t box[4] = {32, (uint32_t)kWtChunk, 1, 1};
-    return encode_map(m, base, 4, dims, strides, box, 1, 4);
+    return encode_map(m, base, 4, dims, strides, box, 0, 4);
 }
 
 bool wgrad_tc_eligible(const aero_tapgemm_params& p, const void* a1, const void* a2, const void* dy) {
@@ -242,10 +235,10 @@ int wgrad_tc_launch(const float* a1, const float* a2, const float* dy, float* dw
     g.dw = dw; g.p = p; g.dw_sn = dw_sn; g.dw_sk = dw_sk; g.dw_ss = dw_ss;
     g.tiles_t = cdiv(p.T, kWtChunk);
     g.n_tiles = cdiv(p.N, 128);
-    // B tile = up to eight 32-channel boxes taken from the concatenation of the two sources (a box never straddles them)
+    // B tile = up to kWtMaxBoxes 32-channel boxes taken from the concatenation of the two sources (a box never straddles them)
     g.nb1 = cdiv(p.C1, 32);
     g.nb = g.nb1 + cdiv(p.C2, 32);
-    g.k_tiles = cdiv(g.nb, 8);
+    g.k_tiles = cdiv(g.nb, kWtMaxBoxes);
     g.bpt = cdiv(g.nb, g.k_tiles);
     g.BN = 32 * g.bpt;
     CUtensorMap mA1, mA2, mDy;
@@ -255,15 +248,9 @@ int wgrad_tc_launch(const float* a1, const float* a2, const float* dy, float* dw
     if (!p.C1) mA1 = mA2;
     if (!p.C2) mA2 = mA1;
     if ((rc = wt_map(&mDy, dy, p.N, p.T, p.F_out, p.B, p.o_sb, p.o_sf, p.o_st)) != AERO_OK) return rc;
-    g.tmem_cols = 32;
-    while ((int)g.tmem_cols < g.BN) g.tmem_cols <<= 1;
-    // instruction descriptor: D = F32, A / B = TF32, both MN-major (bits 15, 16), N = BN, M = 128
-    g.idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(g.BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
     const int stage_bytes = kWtATile + (g.BN / 32) * 4096;
     const int fixed = (int)sizeof(WgradTcShared) + 1024;
-    g.stages = (226 * 1024 - fixed) / stage_bytes;
-    if (g.stages > kWtMaxStages) g.stages = kWtMaxStages;
-    if (g.stages < 2) g.stages = 2;
+    g.stages = 3;                                 // ~97 KB with barriers and alignment: two CTAs per SM, one's fragment loads overlap the other's MMAs
     const size_t smem = (size_t)g.stages * stage_bytes + fixed;
     const int nslab = (p.mode == AERO_TAPS_CONVT) ? p.kf : p.kf * p.kt;
     const int64_t n_chunks = (int64_t)p.B * p.F_out * g.tiles_t;
@@ -274,11 +261,12 @@ int wgrad_tc_launch(const float* a1, const float* a2, const float* dy, float* dw
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
     }
-    // split the pixel axis: one CTA per SM is resident (the pipeline takes the shared memory), so the grid should be a whole number of
+    // split the pixel axis: two CTAs per SM are resident (the pipeline takes the shared memory), so the grid should be a whole number of
     // waves.  Among the split counts that give 2 .. 6 waves pick the one with the fullest last wave; a split keeps at least 8 chunks so
     // that the atomics stay a small fraction of the work.
     const int64_t max_splits = n_chunks / 8 > 0 ? n_chunks / 8 : 1;
-    int64_t lo = cdiv((int64_t)2 * num_sms, items), hi = cdiv((int64_t)6 * num_sms, items);
+    const int64_t slots = (int64_t)2 * num_sms;
+    int64_t lo = cdiv(2 * slots, items), hi = cdiv(6 * slots, items);
     if (lo > max_splits) lo = max_splits;
     if (hi > max_splits) hi = max_splits;
     if (hi > 65535) hi = 65535;
@@ -288,7 +276,7 @@ int wgrad_tc_launch(const float* a1, const float* a2, const float* dy, float* dw
     double best_eff = 0.0;
     for (int64_t sp = lo; sp <= hi; ++sp) {
         const int64_t ctas = items * sp;
-        const double eff = (double)ctas / (double)(cdiv(ctas, (int64_t)num_sms) * num_sms);
+        const double eff = (double)ctas / (double)(cdiv(ctas, slots) * slots);
         if (eff > best_eff + 0.02) { best_eff = eff; splits = sp; }      // prefer fewer splits unless clearly fuller
     }
     g.splits = (int)splits;
@@ -296,11 +284,11 @@ int wgrad_tc_launch(const float* a1, const float* a2, const float* dy, float* dw
     const int d_row = g.splits / g.tiles_t;
     g.d_fo = d_row % p.F_out;
     g.d_b = d_row / p.F_out;
-    if (nslab > 65535 || items / nslab > 2147483647LL) { set_error("aero_tapgemm_wgrad(tcgen05): grid too large"); return AERO_ERR_INVALID; }
+    if (nslab > 65535 || items / nslab > 2147483647LL) { set_error("aero_tapgemm_wgrad(tensor cores): grid too large"); return AERO_ERR_INVALID; }
     cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     dim3 grid((unsigned)(items / nslab), (unsigned)nslab, (unsigned)splits);
     wgrad_tc_kernel<<<grid, kWtThreads, smem, st>>>(mA1, mA2, mDy, g);
-    return check_launch("aero_tapgemm_wgrad(tcgen05)");
+    return check_launch("aero_tapgemm_wgrad(tensor cores)");
 }
 
 }  // namespace aero

@@ -46,7 +46,7 @@ def tf32_round(t):
 
 
 def lstm_gate_reorder(H):
-    """Row order of the tcgen05 LSTM recurrence (csrc/lstm_tc.cu): 4/GPT tiles of 128 rows per direction.
+    """Row order of the wgmma LSTM recurrence (csrc/lstm_tc.cu): 4/GPT tiles of 128 rows per direction.
     GPT=1 (H > 64): tile g = gate g, lane = cell.  GPT=2 (H <= 64): tile t = gates (2t, 2t+1); in each 32-lane
     group lanes 0-15 carry gate 2t and lanes 16-31 gate 2t+1 of the same 16 cells.
     Returns (source row in PyTorch's [i|f|g|o] x H order, validity mask)."""
@@ -64,7 +64,7 @@ def lstm_gate_reorder(H):
 
 
 def lstm_whh_fp16(whh_rows):
-    """[rows, H] fp32 -> [rows, 64*ceil(H/64)] fp16 (zero padded): the A operand of the tcgen05 LSTM recurrence."""
+    """[rows, H] fp32 -> [rows, 64*ceil(H/64)] fp16 (zero padded): the A operand of the wgmma LSTM recurrence."""
     rows, H = whh_rows.shape
     out = torch.zeros(rows, 64 * ((H + 63) // 64), dtype=torch.float16, device=whh_rows.device)
     out[:, :H] = whh_rows.to(torch.float16)
@@ -72,7 +72,7 @@ def lstm_whh_fp16(whh_rows):
 
 
 def pack_kmajor_fp16(w_tkn):
-    """[taps, K, pad4(N)] fp32 -> [taps, pad4(N), pad8(K)] fp16: the kind::f16 tcgen05 weight layout (16-byte rows for TMA)."""
+    """[taps, K, pad4(N)] fp32 -> [taps, pad4(N), pad8(K)] fp16: the f16 wgmma weight layout (16-byte rows for TMA)."""
     taps, k, n = w_tkn.shape
     out = torch.zeros(taps, n, (k + 7) & ~7, dtype=torch.float16, device=w_tkn.device)
     out[:, :, :k] = w_tkn.permute(0, 2, 1).to(torch.float16)
@@ -124,24 +124,23 @@ class AeroEngine:
         self._plist = None
         self._windows = {}
         self._stats = None
-        # 2 (default): FP16-stored activations / tcgen05 kind::f16 operands, fp32 accumulate, fp32 GroupNorm inputs and
+        # 2 (default): FP16-stored activations / f16 wgmma operands, fp32 accumulate, fp32 GroupNorm inputs and
         #    gate pre-activations -- TF32's 10-bit mantissa at half the HBM bytes and twice the tensor-core rate;
-        # 1: fp32-stored activations rounded to TF32 / tcgen05 kind::tf32;  0: exact fp32 SIMT kernels everywhere.
+        # 1: fp32-stored activations rounded to TF32 / tf32 wgmma;  0: exact fp32 SIMT kernels everywhere.
         self.precision = 2
         # alternate the walk direction of consecutive tap-GEMM / norm_act launches (AERO_TG_REVERSE) so that a consumer starts
-        # on what its producer wrote last; measured on B200: no gain for this model (12.19 ms either way), so off
+        # on what its producer wrote last; off by default (its effect has not been measured on H100)
         self.snake = False
         self._flip = False
         # precision 2 only: pre-normalisation GEMM outputs (GroupNorm inputs) are stored in FP16 as well; their statistics are
         # taken from the stored values.  Halves the bytes of every norm_act pass and of the GEMM writes that feed them
         # (tests/err_budget_emu.py: +6 % end-to-end error, paid for by keeping the last decoder layer's GLU output in fp32)
         self.raw16 = True
-        # precision 2 + tcgen05 LSTM: optionally store the gate pre-activations (input projections, 8H columns per frame) in FP16
-        # too.  Accuracy-neutral (tests/err_budget_emu.py) but measured SLOWER on B200: the recurrence reads them with scalar
-        # loads (one gate of one cell per lane), and 2-byte loads cost 307 -> 336 us per H = 96 launch while the projection
-        # GEMMs gain only ~0.05 ms per step (tools/kprof.py lstm96 / lstm48, round 2) -- off.
+        # precision 2 + wgmma LSTM: optionally store the gate pre-activations (input projections, 8H columns per frame) in FP16
+        # too.  Accuracy-neutral (tests/err_budget_emu.py); the recurrence reads them with scalar loads (one gate of one cell
+        # per lane), which 2-byte elements do not make cheaper, so off by default (not measured on H100).
         self.gin16 = False
-        self.lstm_tc = True         # tcgen05 LSTM recurrence (re-ordered gate layout) when precision >= 1
+        self.lstm_tc = True         # wgmma LSTM recurrence (re-ordered gate layout) when precision >= 1
         self.fuse_pre_ftb = True    # encoder layer 0: evaluate FTB through the linear pre_conv (csrc/ftb_lin.cu)
         self.fp32_tags = ()         # tap-GEMM tags (prefix match) forced onto the exact-fp32 path even when precision == 1
         self._prof, self._prof_tags = None, set()
@@ -197,7 +196,7 @@ class AeroEngine:
         dev = self._device()
         if dev.type != "cuda" or not x.is_cuda:
             raise RuntimeError(
-                "aero_b200.Aero runs on CUDA only (sm_100a kernels in libaero_b200.so); there is no CPU path. "
+                "aero_b200.Aero runs on CUDA only (sm_90a kernels in libaero_b200.so); there is no CPU path. "
                 f"model on {dev}, input on {x.device}")
         if x.device != dev:
             raise RuntimeError(f"input on {x.device} but model on {dev}")
@@ -323,7 +322,7 @@ class AeroEngine:
                                 sd[f"{q}.lstm.lstm.bias_ih_l{l}_reverse"] + sd[f"{q}.lstm.lstm.bias_hh_l{l}_reverse"]]).contiguous()
                             W[f"{o}.lstm{l}.whh"] = torch.stack([sd[f"{q}.lstm.lstm.weight_hh_l{l}"],
                                                                   sd[f"{q}.lstm.lstm.weight_hh_l{l}_reverse"]]).contiguous()
-                        # tcgen05 recurrence: gate rows re-ordered / padded (include/aero_b200.h, aero_lstm_params.precision)
+                        # wgmma recurrence: gate rows re-ordered / padded (include/aero_b200.h, aero_lstm_params.precision)
                         H_ = sd[f"{q}.lstm.lstm.weight_hh_l0"].shape[1]
                         src, ok = (t_.to(dev) for t_ in lstm_gate_reorder(H_))
                         for l in range(2):
@@ -357,8 +356,8 @@ class AeroEngine:
             W[p + ".ct.w"] = pack_taps(sd[p + ".conv_tr.weight"][:, :, :, 0].permute(1, 0, 2))
             W[p + ".ct.b"] = sd[p + ".conv_tr.bias"].contiguous()
         out = {k: (v.to(dev) if v.dtype == torch.float16 else v.to(device=dev, dtype=torch.float32)) for k, v in W.items()}
-        # K-major TF32 twins of every tap-GEMM weight for the tcgen05 path: [taps, K, pad4(N)] -> [taps, pad4(N), K]
-        # ... and FP16 twins [taps, pad4(N), pad8(K)] for kind::f16
+        # K-major TF32 twins of every tap-GEMM weight for the wgmma path: [taps, K, pad4(N)] -> [taps, pad4(N), K]
+        # ... and FP16 twins [taps, pad4(N), pad8(K)] for the f16 wgmma
         self._wk, self._wh, self._wname = {}, {}, {}
         for k in [k for k in out if k.endswith("ftbfc.w")]:
             out[k + "@k"] = tf32_round(out[k])          # [F', F] is already K-contiguous
@@ -399,7 +398,7 @@ class AeroEngine:
         p = cabi.TapGemmParams(B, F_out, T, N, F_in, T_in, C1, C2, mode, kf, kt, stride_f, pad_f, dil_t, pad_t, f_off,
                                act, glu, stats_mode, groups, *a1_s, *a2_s, w_sb, *o_s, *r_s, *cs_s, 0, flags)
         if mode == cabi.TAPS_MIX:
-            p.precision = 2 if a16 else 1        # tcgen05-only mode; `w` is already the K-major twin of the right kind
+            p.precision = 2 if a16 else 1        # wgmma-only mode; `w` is already the K-major twin of the right kind
         elif self.precision >= 1 and w_sb == 0 and not (tag and self.fp32_tags and tag.startswith(self.fp32_tags)):
             wk = (self._wh if a16 else self._wk).get(w.data_ptr())
             if wk is not None and self.lib.aero_tapgemm_tc_eligible(C.byref(p)):
@@ -615,7 +614,7 @@ class AeroEngine:
         n_seq = rows * n_win
         tc = self.lstm_tc and self.precision >= 1 and H % 4 == 0 and 32 < H <= 96
         # the input projections use PyTorch's own [dir][i,f,g,o][H] column order on both paths; only W_hh is re-ordered
-        # (tile / lane order, FP16) for the tcgen05 recurrence
+        # (tile / lane order, FP16) for the wgmma recurrence
         G = 8 * H
         whh0, whh1 = (W[f"{o}.lstm0r.whh"], W[f"{o}.lstm1r.whh"]) if tc else (W[f"{o}.lstm0.whh"], W[f"{o}.lstm1.whh"])
         gdt = torch.float16 if (tc and self.precision == 2 and self.gin16 and h.dtype == torch.float16) else torch.float32

@@ -5,7 +5,7 @@ the reference's Python surface (reference ``src/models/aero.py:223-268`` ctor
 kwargs, ``:446`` ``forward(mix, return_spec, return_lr_spec)``, ``:409``
 ``_spec(x, scale)``, the 331-key ``state_dict`` layout and
 ``_init_args_kwargs`` used by ``src/model_serializer.py:20``) while the
-arithmetic is executed by the sm_100a kernels in ``aero_b200/csrc`` through the
+arithmetic is executed by the sm_90a kernels in ``aero_b200/csrc`` through the
 C-ABI library (``include/aero_b200.h``).
 
 The module tree below only *holds parameters*; none of the ``nn`` layers'
@@ -239,7 +239,7 @@ class _AeroTrainFn(torch.autograd.Function):
     def forward(ctx, mix, model, names, *params):
         from .train_engine import TrainEngine
         if not mix.is_cuda or next(model.parameters()).device != mix.device:
-            raise RuntimeError("aero_b200.Aero trains on CUDA only (sm_100a kernels in libaero_b200.so); there is no CPU path")
+            raise RuntimeError("aero_b200.Aero trains on CUDA only (sm_90a kernels in libaero_b200.so); there is no CPU path")
         with torch.cuda.device(mix.device):
             eng = TrainEngine(model)
             wave, spec = eng.forward(mix)
@@ -256,7 +256,7 @@ class _AeroTrainFn(torch.autograd.Function):
 
 
 class Aero(nn.Module):
-    """AERO generator (audio super-resolution in the spectral domain), B200-native.
+    """AERO generator (audio super-resolution in the spectral domain), H100-native (sm_90a).
 
     Constructor kwargs, defaults and attribute names follow reference
     ``src/models/aero.py:223-268`` so that ``Aero(**args.experiment.aero)``

@@ -52,7 +52,7 @@ class TrainEngine:
         # Arithmetic of the convolutions' forward, data-gradient and weight-gradient GEMMs (normalisation, LSTM recurrence, attention and
         # all reductions are fp32 / fp64 in every mode):
         #   0  exact-fp32 SIMT tap-GEMMs (the original gradient-parity mode);
-        #   1  TF32 on the tcgen05 tensor cores (what cuDNN does for the reference under PyTorch's default cudnn.allow_tf32);
+        #   1  TF32 on the tensor cores (what cuDNN does for the reference under PyTorch's default cudnn.allow_tf32);
         #   3  "3xTF32": every operand split into hi + lo TF32 halves, three tensor-core products hi*hi + hi*lo + lo*hi summed in fp32 --
         #      fp32-grade results (~2^-22 per product) at tensor-core speed.
         self.precision = int(getattr(model, "train_precision", 0))
@@ -164,7 +164,7 @@ class TrainEngine:
     def _gemm_call(self, p, out, w, a1=None, a2=None, bias=None, residual=None, samp_affine=None, stats=None, colscale=None, halves=None):
         """aero_tapgemm_fwd in the engine's arithmetic mode.  halves: optional dict id(tensor) -> (hi, lo) of operands already split."""
         if p.precision in (1, 3):
-            # tcgen05 path: K-major TF32 twin [taps, pad4(N), K] of the packed weight [taps, K, pad4(N)]; shapes it does not take stay SIMT
+            # wgmma path: K-major TF32 twin [taps, pad4(N), K] of the packed weight [taps, K, pad4(N)]; shapes it does not take stay SIMT
             ok = p.w_sb == 0 and colscale is None and w.dim() == 3 and bool(self.lib.aero_tapgemm_tc_eligible(C.byref(p)))
             if ok and p.precision == 3:
                 ok = self._splittable(a1, p.C1, p.a1_sb, p.a1_sf, p.a1_st, p) and self._splittable(a2, p.C2, p.a2_sb, p.a2_sf, p.a2_st, p)

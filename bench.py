@@ -2,6 +2,7 @@
 """bench.py -- audio-seconds/sec of the AERO generator forward (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 4-16|12-48|11-44|train]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one forward over one batch of synthetic white-noise clips per GPU; clips are independent, so ranks shard
@@ -17,12 +18,14 @@ the batch with no data-path collective ("weak" scaling: the per-GPU batch is fix
   e2e      : same metric through the public API with pinned-host input, H2D and D2H of the waveform inside the timed
              region; median of the per-step times (mean also given).
   roofline : dominant kernel family = the decoder's 3x3 rewrite tap-GEMMs, timed with CUDA events on the launch stream
-             in a separate eager pass of the same K steps; fraction of the measured burst AND sustained cuBLAS bf16 rates.
+             in a separate eager pass of the same K steps; fraction of the H100 SXM data-sheet dense rate.
+  --dump-outputs DIR : after the timed steps, what the last timed step returned goes to DIR/<name>.npy (float32): the waveform,
+             or for --config train the loss and the updated generator parameters.  Inputs are seeded, so two builds can be
+             compared output for output.
   step     : whole-step achieved TFLOP/s against the same peaks, and the step time against the sum of its launches' own
              rooflines (tools/traffic_model.py: algorithmic bytes / FLOPs per launch).
   cpu_baseline / --impl reference : the oracle port (oracle/aero_oracle.py, the same torch library calls the reference
-             makes) on the host cores, BASELINE.md section 3 protocol.  The reference is a Python package and cannot travel
-             to the GPU box; oracle/ is its pinned restatement.
+             makes) on the host cores, BASELINE.md section 3 protocol; oracle/ is the reference's pinned restatement.
 """
 import argparse
 import json
@@ -51,25 +54,15 @@ CONFIGS = {
                   name="aero_11-44_512_64 inference forward, 10 s stereo white-noise clips 11.025->44.1 kHz (BASELINE configs[4]: "
                        "8 clips on 4 GPUs = 2 per GPU)"),
 }
-# dram__bytes_read.sum + dram__bytes_write.sum of the largest launch of the roofline family (decoder.0 rewrite, B=32) from the
-# `ncu --set full` capture summarised in profiles/
-TRAFFIC_NCU = {1: {"kernel": "tapgemm_tc_kernel<0,0,1,tf32> decoder.0.rw B=32", "bytes_per_launch": 473.8e6, "algorithmic_bytes": 513.7e6,
-                   "tensor_pipe_pct": 80.8, "source": "profiles/r1_dec0rw_tc_ncu.md"},
-               2: {"kernel": "tapgemm_tc_kernel<0,0,1,f16,f16> decoder.0.rw B=32", "bytes_per_launch": 208.2e6, "algorithmic_bytes": 256.9e6,
-                   "tensor_pipe_pct": 89.5, "source": "profiles/r2_dec0rw_f16_ncu.md"}}
-
 
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        d = json.load(open(path))
-        return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops_sustained"], "bf16_tflops_burst": d["bf16_tflops"],
-                "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "bf16_tflops_burst": 1650.0, "source": "fallback (B200_PROFILING.md)"}
+    """Denominators of the roofline fractions: NVIDIA's data-sheet figures for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 TFLOP/s
+    dense FP16 / BF16.  They are bounds, not measurements; a power-limited card sustains less."""
+    return {"hbm_gbs": 3350.0, "fp16_tflops": 989.0, "source": "H100 SXM data sheet (700 W)"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -249,6 +242,21 @@ def run_reference(args, cfg, rank, world):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(directory, arrays, limit_bytes=64 << 20):
+    """DIR/<name>.npy, float32, for each array a caller of the timed path receives; together at most `limit_bytes`: a larger
+    array is stored as a fixed, seeded sample of its positions."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    share = limit_bytes // (4 * len(arrays))
+    for name, t in arrays.items():
+        flat = t.detach().float().reshape(-1).cpu()
+        if flat.numel() > share:
+            flat = flat[torch.randint(0, flat.numel(), (share,), generator=torch.Generator().manual_seed(SEED))]
+            np.save(os.path.join(directory, name + ".npy"), flat.numpy())
+        else:
+            np.save(os.path.join(directory, name + ".npy"), flat.numpy().reshape(tuple(t.shape)))
+
+
 def timed_steps(fn, steps, barrier):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
@@ -271,10 +279,14 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the precision sub-lines and the strong-scaling sample")
     ap.add_argument("--precision", type=int, default=None,
-                    help="engine precision: 2 (default) FP16-stored activations / kind::f16 tcgen05, 1 fp32 storage / kind::tf32, "
+                    help="engine precision: 2 (default) FP16-stored activations / f16 wgmma, 1 fp32 storage / tf32 wgmma, "
                          "0 every kernel in exact fp32")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned to DIR/<name>.npy (float32, at most 64 MB: a seeded sample beyond that)")
     ap.add_argument("--_cpu_probe", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs stores what the GPU path computed; it does not apply to --impl reference")
     if args.config == "train":
         import bench_train
         return bench_train.main(args)
@@ -332,7 +344,10 @@ def main():
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    ms_dev = timed_steps(lambda: model(x_dev), args.steps, barrier)
+    last = {}
+    ms_dev = timed_steps(lambda: last.__setitem__("out", model(x_dev)), args.steps, barrier)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"waveform" if world == 1 else f"waveform_rank{rank}": last["out"]})
 
     # ---- the same K steps launched eagerly with CUDA events around the roofline kernel family
     fam = ("decoder.0.rw", "decoder.1.rw", "decoder.2.rw", "decoder.3.rw")      # tags = packed-weight names
@@ -371,7 +386,7 @@ def main():
             eng.use_graph = False
             model(x_dev)
             extras[f"precision_{prec}"] = {"ms_per_step": timed_steps(lambda: model(x_dev), 3, barrier),
-                                           "what": {1: "fp32 storage rounded to TF32 / tcgen05 kind::tf32", 0: "every kernel in exact fp32 (SIMT)"}[prec]}
+                                           "what": {1: "fp32 storage rounded to TF32 / tf32 wgmma", 0: "every kernel in exact fp32 (SIMT)"}[prec]}
         eng.precision, eng.use_graph = keep, "auto"
         if world > 1 and B % world == 0:
             # strong scaling sample: the ONE-GPU workload (B clips in total) split over the ranks
@@ -399,36 +414,33 @@ def main():
         n_l = sum(v["launches"] for v in prof.values())
         prec = eng.precision
         tf32 = prec == 1
-        # kind::f16 runs at the bf16 rate the driver measured with cuBLAS; kind::tf32 at half of it (no TF32 figure is measured)
+        # f16 operands run at the data sheet's FP16 / BF16 rate, tf32 operands at half of it
         div = 2 if tf32 else 1
-        peak_s, peak_b = pk["bf16_tflops"] / div, pk["bf16_tflops_burst"] / div
+        peak = pk["fp16_tflops"] / div
         clk = sampler.summary()
-        pipe = (4096 if tf32 else 8192) * 148 * (clk.get("sm_mhz") or 1965) * 1e6 / 1e12     # tcgen05 flop/clk/SM (ncu pipe rate)
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        pipe = (2048 if tf32 else 4096) * sms * (clk.get("sm_mhz") or clk.get("sm_max_mhz") or 1980) * 1e6 / 1e12     # wgmma flop/clk/SM
         ach = flops / (ms_k * 1e-3) / 1e12 if ms_k > 0 else 0.0
         roof = {"bound": "tensor", "kernel": "tap-GEMM, decoder 3x3 rewrite convs (4 launches/step)",
-                "achieved": ach, "peak": peak_b, "unit": "TFLOP/s", "frac": ach / peak_b,
-                "frac_burst": ach / peak_b, "frac_sustained": ach / peak_s, "peak_sustained": peak_s,
-                "peak_source": pk["source"] + ": cuBLAS bf16 8192^3 best-of-10 (burst; the family is a ~16 % duty cycle of a step at max "
-                               "clock, so burst is the denominator of `frac`) and back-to-back for 4 s (sustained)" +
-                               ("; TF32 dense peak taken as half the bf16 figure" if tf32 else "; cuBLAS bf16 = the kind::f16 rate") +
+                "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
+                "peak_source": pk["source"] + (": dense TF32" if tf32 else ": dense FP16") +
                                "; frac_tensor_pipe is the stricter fraction of the tensor pipe's own rate at the sampled clock",
                 "peak_tensor_pipe": pipe, "frac_tensor_pipe": ach / pipe,
-                "precision": {2: "f16 operands tcgen05 (kind::f16), fp32 accumulate", 1: "tf32 tcgen05", 0: "fp32 SIMT (no tensor pipe)"}[prec],
+                "precision": {2: "f16 operands (wgmma), fp32 accumulate", 1: "tf32 wgmma", 0: "fp32 SIMT (no tensor pipe)"}[prec],
                 "ms_per_step_in_kernel": ms_k / args.steps, "share_of_step": (ms_k / args.steps) / ms_eager,
                 "timed_in": "eager pass of the same K steps (CUDA events on the launch stream around each launch of the family)",
                 "launches_timed": n_l,
-                "per_layer_tflops": {k: (v["flops"] / (v["ms"] * 1e-3) / 1e12 if v["ms"] > 0 else 0.0) for k, v in sorted(prof.items())},
-                "traffic": TRAFFIC_NCU.get(prec) if args.config == "4-16" else None}
+                "per_layer_tflops": {k: (v["flops"] / (v["ms"] * 1e-3) / 1e12 if v["ms"] > 0 else 0.0) for k, v in sorted(prof.items())}}
         gflop_req = cfg["gflop_req"] or cfg["gflop"]
         step_tflops = B * gflop_req * 1e9 / (ms_dev * 1e-3) / 1e12
-        step = {"tflops": step_tflops, "frac_sustained": step_tflops / peak_s, "frac_burst": step_tflops / peak_b,
+        step = {"tflops": step_tflops, "frac": step_tflops / peak,
                 "gflop_per_clip_counted": gflop_req}
         try:
             import traffic_model
-            sr = traffic_model.step_roofline(cfg["exp"], B, L, prec, p_tensor=peak_s * 1e12)
+            sr = traffic_model.step_roofline(cfg["exp"], B, L, prec, p_tensor=peak * 1e12)
             step.update({"sum_of_launch_rooflines_ms": sr["sum_roofline_ms"], "frac_of_sum_of_rooflines": sr["sum_roofline_ms"] / ms_dev,
                          "algorithmic_hbm_gb_per_step": sr["hbm_gb"], "avg_hbm_tbs": sr["hbm_gb"] / ms_dev,
-                         "how": "tools/traffic_model.py: per launch max(read/5.55, write/3.88, (r+w)/6.49 TB/s, FLOP/sustained peak), summed"})
+                         "how": "tools/traffic_model.py: per launch max(bytes / 3.35 TB/s, FLOP / data-sheet peak), summed"})
         except Exception as e:          # the model is tooling; the bench line does not depend on it
             step["sum_of_launch_rooflines_ms"] = None
             step["traffic_model_error"] = str(e)[:200]
@@ -438,7 +450,7 @@ def main():
                           1: "f32 (tf32 tensor-core operands, fp32 accumulate)", 0: "f32"}[prec], "data": "synthetic",
                 "config": {"workload": f"{cfg['name']}, batch {B}/GPU", "config_key": args.config,
                            "global_batch": total_clips, "parallelism": f"batch-sharded x{world}, no collective",
-                           "l2": "activations (>700 MB/step) exceed the 126 MB L2; no explicit flush",
+                           "l2": "activations (>700 MB/step) exceed the 50 MB L2; no explicit flush",
                            "gflop_per_clip": cfg["gflop"], "gflop_per_clip_required": gflop_req,
                            "timed_path": "CUDA-graph replay (what Aero.forward does for a steady-state shape)",
                            "host_numa_cores": numa_cores},

@@ -137,6 +137,10 @@ def main(args):
     ar0 = trainer.allreduce_bytes
     ms_dev = B.timed_steps(lambda: losses.append(one_step(lr_d, hr_d)), args.steps, barrier)
     launches = lib.aero_launch_count() - l0
+    if args.dump_outputs:           # what the last timed step produced: its loss and the parameters it left behind
+        sfx = "" if world == 1 else f"_rank{rank}"
+        B.dump_outputs(args.dump_outputs, {"loss" + sfx: torch.as_tensor(losses[-1]).reshape(1),
+                                           "generator_parameters" + sfx: torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])})
     ar_bytes = (trainer.allreduce_bytes - ar0) / args.steps
     sampler.paused = True
     barrier()
@@ -174,15 +178,15 @@ def main(args):
         pk = B.peaks()
         total = bsz * world
         value = total * SECONDS / (ms_dev * 1e-3)
-        fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12                           # SIMT fp32 FMA peak of a B200 at max clock, TFLOP/s
+        fp32_peak = 132 * 128 * 2 * 1.98e9 / 1e12                            # SIMT fp32 FMA peak of an H100 SXM at 1980 MHz, TFLOP/s
         step_tflops = bsz * 3 * GFLOP_FWD * 1e9 / (ms_dev * 1e-3) / 1e12
         first, last = float(losses[0]), float(losses[-1])
         line = {"metric": "audio-seconds/sec training step", "value": value, "unit": "audio-s/s", "n_gpus": world, "steps": args.steps,
                 "warmup": warm, "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": {0: "f32 (exact-fp32 SIMT tap-GEMMs for forward, dgrad and wgrad; fp64 reduction accumulators)",
-                          3: "f32-grade: 3xTF32 tensor-core GEMMs (tcgen05, hi/lo operand split, fp32 accumulate) for the convolutions' forward, dgrad, "
+                          3: "f32-grade: 3xTF32 tensor-core GEMMs (tensor cores, hi/lo operand split, fp32 accumulate) for the convolutions' forward, dgrad, "
                              "wgrad; fp32 SIMT everything else; fp64 reduction accumulators",
-                          1: "tf32 tensor-core GEMMs (tcgen05: forward, dgrad, wgrad of the convolutions), fp32 everything else, fp64 reduction "
+                          1: "tf32 tensor-core GEMMs (wgmma: forward, dgrad, wgrad of the convolutions), fp32 everything else, fp64 reduction "
                              "accumulators"}[train_precision],
                 "data": "synthetic",
                 "config": {"workload": f"{EXP} training step (G + MelGAN-D + MR-STFT, Adam: reference adversarial config), batch {bsz}/GPU "
@@ -191,21 +195,21 @@ def main(args):
                            "adversarial": bool(adversarial), "train_precision": train_precision,
                            "step": ("generator forward (train) + MR-STFT + 3 MelGAN-discriminator forwards + G backward + Adam + D backward + Adam"
                                     if adversarial else "generator forward (train) + MR-STFT + backward + Adam"),
-                           "l2": "activations saved for backward (~1 GB/step) exceed the 126 MB L2; no explicit flush"},
+                           "l2": "activations saved for backward (~1 GB/step) exceed the 50 MB L2; no explicit flush"},
                 "e2e": {"value": total * SECONDS / (ms_e2e * 1e-3), "unit": "audio-s/s", "ms_per_step": ms_e2e,
                         "statistic": "median of per-step device times (H2D of lr+hr, step, D2H of the loss, one stream sync per step)",
                         "h2d_bytes_per_step": (host_lr.numel() + host_hr.numel()) * 4 * world, "d2h_bytes_per_step": 4 * world},
                 "gpu_launches": int(launches), "allreduce_bytes_per_step_per_rank": ar_bytes,
                 "loss_first_last": [first, last], "clocks": sampler.summary(),
                 "roofline": {"bound": "tensor", "kernel": "whole step (forward + dgrad + wgrad tap-GEMMs dominate)", "achieved": step_tflops,
-                             "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": step_tflops / pk["bf16_tflops"],
+                             "peak": pk["fp16_tflops"], "unit": "TFLOP/s", "frac": step_tflops / pk["fp16_tflops"],
                              "frac_of_fp32_simt_peak": step_tflops / fp32_peak, "fp32_simt_peak": fp32_peak,
                              "note": "convolution GEMMs: see dtype; LSTM recurrence, attention, normalisation and the grouped discriminator convolutions "
                                      "are fp32 SIMT in every mode; `other_modes` times the same step in the other arithmetic modes", "traffic": None}}
         what = {0: "model.train_precision = 0: exact-fp32 SIMT GEMMs",
                 3: "model.train_precision = 3 (3xTF32): every convolution GEMM (forward, dgrad, wgrad) as three TF32 tensor-core products on hi / lo "
                    "operand halves, fp32-grade results; meets the exact mode's gradient-parity bars (tests/test_gpu_train_tc.py)",
-                1: "model.train_precision = 1: the convolution GEMMs in plain TF32 on tcgen05 (what cuDNN does for the reference under PyTorch's "
+                1: "model.train_precision = 1: the convolution GEMMs in plain TF32 on wgmma (what cuDNN does for the reference under PyTorch's "
                    "default allow_tf32); all-gradient deviation from the fp64 reference 6.5e-2, the reference algorithm under PyTorch-default TF32 "
                    "on the same GPU 5.3e-2 (tests/test_gpu_train_tc.py)"}
         if ms_others:

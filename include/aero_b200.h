@@ -1,5 +1,5 @@
 /*
- * aero_b200.h -- C ABI of libaero_b200.so: the sm_100a kernels behind the AERO generator forward.
+ * aero_b200.h -- C ABI of libaero_b200.so: the sm_90a kernels behind the AERO generator forward.
  *
  * The reference (slp-rl/aero) has no FFI: its hot path is the Python class
  * src/models/aero.py:218 `Aero`, whose arithmetic is dispatched to PyTorch library kernels.
@@ -40,7 +40,7 @@ enum aero_status {
 
 int aero_abi_version(void);            /* 3: training entry points */
 const char* aero_last_error(void);
-/* compute capability of the current device as 10*major+minor (100 on B200); <0 if no device */
+/* compute capability of the current device as 10*major+minor (90 on H100); <0 if no device */
 int aero_device_arch(void);
 /* number of kernel launches issued through this library by the calling process (bench.py's gpu_launches) */
 uint64_t aero_launch_count(void);
@@ -139,8 +139,8 @@ typedef struct {
     int64_t r_sb, r_sf, r_st;         /* residual strides */
     int64_t cs_sb, cs_st;             /* colscale strides */
     int32_t precision;                /* 0: fp32 SIMT tiles, fp32 weights N-contiguous  W[slab][K][pad4(N)] (sources / outputs of either type);
-                                         1: tcgen05 kind::tf32, fp32 sources, fp32 weights K-contiguous W[slab][pad4(N)][K] rounded to TF32;
-                                         2: tcgen05 kind::f16, FP16 sources, FP16 weights K-contiguous W[slab][pad4(N)][pad8(K)];
+                                         1: wgmma kind::tf32, fp32 sources, fp32 weights K-contiguous W[slab][pad4(N)][K] rounded to TF32;
+                                         2: wgmma kind::f16, FP16 sources, FP16 weights K-contiguous W[slab][pad4(N)][pad8(K)];
                                             1 / 2: AERO_ERR_UNSUPPORTED unless aero_tapgemm_tc_eligible() */
     int32_t flags;                    /* AERO_TG_* */
 } aero_tapgemm_params;
@@ -151,15 +151,15 @@ enum {
     AERO_TG_ROUND_TF32 = 1,           /* fp32 outputs: round stored values to TF32 (round-to-nearest) for a kind::tf32 consumer */
     AERO_TG_A_F16 = 2,                /* a1 / a2 are FP16 */
     AERO_TG_OUT_F16 = 4,              /* out and residual are FP16 */
-    AERO_TG_REVERSE = 8               /* tap-GEMM (tcgen05 path) / norm_act: walk tiles / rows from the end.  Results are identical;
+    AERO_TG_REVERSE = 8               /* tap-GEMM (wgmma path) / norm_act: walk tiles / rows from the end.  Results are identical;
                                          a kernel launched right after its producer then starts on the data the producer wrote last,
-                                         which is still in the 126 MB L2 (the host alternates the direction from launch to launch) */
+                                         which is still in the 50 MB L2 (the host alternates the direction from launch to launch) */
 };
 int aero_tapgemm_fwd(const void* a1, const void* a2, const void* w, const float* bias,
                      const float* addend_fn, const float* colscale, const void* residual,
                      const float* samp_affine, void* out, double* stats,
                      const aero_tapgemm_params* p, aero_stream_t stream);
-/* 1 when the shape can run on the tcgen05 path (kind::tf32, or kind::f16 when flags has AERO_TG_A_F16), else 0 */
+/* 1 when the shape can run on the wgmma path (kind::tf32, or kind::f16 when flags has AERO_TG_A_F16), else 0 */
 int aero_tapgemm_tc_eligible(const aero_tapgemm_params* p);
 
 /* ------------------------------------------------------------------------------------------
@@ -251,7 +251,7 @@ typedef struct {
     int32_t flags;                    /* AERO_TG_ROUND_TF32: round the stored fp32 h to TF32; AERO_TG_OUT_F16: hout is FP16;
                                          AERO_TG_A_F16 (precision 1 only): gin is FP16 (bias_pad stays fp32) */
     int32_t precision;                /* 0: fp32 SIMT recurrence (layouts above);
-                                         1: tcgen05 recurrence, FP16 operands (h in (-1,1), W_hh O(1): same 10-bit mantissa as TF32), fp32
+                                         1: wgmma recurrence, FP16 operands (h in (-1,1), W_hh O(1): same 10-bit mantissa as TF32), fp32
                                             accumulate.  `gin` / `bias_pad` keep the layout above; only `whh` changes: FP16
                                             [2][(4/GPT)*128][Kp], Kp = 64*ceil(H/64), gate rows re-ordered into 4/GPT tiles of 128 per
                                             direction (GPT = 2 if H <= 64 else 1): GPT=1: tile g = gate g, row = cell; GPT=2: tile t =

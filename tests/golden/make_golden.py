@@ -116,7 +116,7 @@ def main():
         y = ref["spec"].ispectro(z, hop, win_length=win)
         blob[f"{i}/params"] = np.array([n_fft, hop, win, L] + list(lead))
         zr = torch.view_as_real(z).reshape(-1)
-        idx = sample_indices(zr.numel(), 32768)
+        idx = sample_indices(zr.numel(), 16384)
         blob[f"{i}/z_idx"] = idx.numpy().astype(np.int32)
         blob[f"{i}/z_val"] = zr[idx].numpy()
         blob[f"{i}/y"] = y.numpy()

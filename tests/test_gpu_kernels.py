@@ -255,7 +255,7 @@ def test_stft_istft_golden_and_roundtrip(golden_dir):
 
 
 # ------------------------------------------------------------------------------------------------
-# tcgen05 path: same contract, TF32 operands.  Inputs are pre-rounded to TF32 so every product is exact
+# wgmma path: same contract, TF32 operands.  Inputs are pre-rounded to TF32 so every product is exact
 # in fp32 and the comparison is tight (it checks descriptors / swizzle / tap geometry, not TF32 noise).
 TC_CASES = [c for c in GEMM_CASES if c[0] not in ("k2_thin_in", "thin_out_relu", "convt_s4_crop_affine")] + [
     ("big_n_tiles", dict(B=1, F_out=2, T=300, N=768, C1=96, kf=3, kt=3, pad_f=1, pad_t=1, stats_mode=1, groups=4)),
@@ -360,7 +360,7 @@ def test_tcgen05_is_selected_for_the_big_convs(engines):
 
 @pytest.mark.parametrize("H,T,rows", [(48, 251, 5), (96, 123, 3), (96, 501, 2), (64, 40, 20), (36, 230, 3)])
 def test_lstm_layer_pair_tcgen05(engines, H, T, rows):
-    """tcgen05 recurrence (TF32 h*W_hh, fp32 accumulate, fast sigmoid/tanh) against the fp32 cell recurrence."""
+    """wgmma recurrence (TF32 h*W_hh, fp32 accumulate, fast sigmoid/tanh) against the fp32 cell recurrence."""
     from aero_b200.engine import lstm_gate_reorder, lstm_whh_fp16, tf32_round
     gpu, emu = engines
     steps, stride, n_win = (200, 100, math.ceil(T / 100)) if T > 200 else (T, 0, 1)
@@ -390,15 +390,15 @@ def test_lstm_layer_pair_tcgen05(engines, H, T, rows):
     finally:
         gpu.precision = 0
     e1, e2 = rel_l2(h1.cpu(), h1c), rel_l2(h2.cpu(), h2c)
-    print(f"lstm tcgen05 H={H} T={T}: rel_l2 {e1:.2e} {e2:.2e}")
+    print(f"lstm wgmma H={H} T={T}: rel_l2 {e1:.2e} {e2:.2e}")
     assert e1 < 1e-3 and e2 < 1e-3
 
 
 @pytest.mark.parametrize("storage", ["tf32", "f16"])
 @pytest.mark.parametrize("B,Fq,T,Cc", [(2, 256, 37, 48), (1, 64, 131, 48), (3, 16, 50, 96), (2, 8, 77, 192)])
 def test_freq_mix_tcgen05_mn_major(engines, B, Fq, T, Cc, storage):
-    """AERO_TAPS_MIX: contraction over the frequency rows with the activations as the MN-major UMMA operand
-    (tf32: SWIZZLE_128B_BASE32B atoms; f16: plain SWIZZLE_128B atoms)."""
+    """AERO_TAPS_MIX: contraction over the frequency rows with the activations as the MN-major wgmma operand
+    (tf32: A fragments loaded into registers from SWIZZLE_128B boxes; f16: transposed-A wgmma on SWIZZLE_128B atoms)."""
     from aero_b200.engine import pack_kmajor_fp16, tf32_round
     gpu, _ = engines
     f16 = storage == "f16"

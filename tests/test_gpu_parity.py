@@ -168,8 +168,8 @@ def test_repeatable_and_buffer_reuse():
 @pytest.mark.parametrize("precision", [2, 1])
 @pytest.mark.parametrize("case", CASES)
 def test_forward_tensor_core_paths_within_tolerance(golden_dir, case, precision):
-    """Tensor-core engines: precision 2 (default; FP16-stored activations, tcgen05 kind::f16, fp32 accumulate, fp32
-    GroupNorm inputs / gate pre-activations) and precision 1 (fp32 storage rounded to TF32, kind::tf32).
+    """Tensor-core engines: precision 2 (default; FP16-stored activations, f16 wgmma, fp32 accumulate, fp32
+    GroupNorm inputs / gate pre-activations) and precision 1 (fp32 storage rounded to TF32, tf32 wgmma).
     north_star bar: 1e-3 relative."""
     g = np.load(os.path.join(golden_dir, case + ".npz"))
     m = build(str(g["exp"])).cuda()
@@ -241,8 +241,8 @@ def test_auto_graph_kicks_in_on_the_third_call_and_matches():
 
 
 def test_faster_than_pytorch_eager_on_the_same_gpu():
-    """SURVEY.md section 8(d): the 'existing Blackwell kernels' to beat are PyTorch's own (cuDNN / cuBLAS / cuFFT) running the
-    same forward on the same B200.  The oracle's library-call form makes exactly the reference's torch calls; here it runs
+    """SURVEY.md section 8(d): the existing kernels to beat are PyTorch's own (cuDNN / cuBLAS / cuFFT) running the
+    same forward on the same GPU.  The oracle's library-call form makes exactly the reference's torch calls; here it runs
     on the GPU (TF32 allowed, as PyTorch's defaults for convolutions) as a timing reference -- it is not on the product path."""
     from oracle import aero_oracle as O
     m = build("aero_4-16_512_64").cuda()

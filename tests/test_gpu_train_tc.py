@@ -1,5 +1,5 @@
 """-m gpu: the TF32 tensor-core training mode (TrainEngine.precision = 1): forward, data-gradient and weight-gradient GEMMs of the
-convolutions on tcgen05 (csrc/tapgemm_tc.cu, csrc/wgrad_tc.cu) against torch autograd in fp64 on the CPU.
+convolutions on the tensor cores (csrc/tapgemm_tc.cu, csrc/wgrad_tc.cu) against torch autograd in fp64 on the CPU.
 
 Tolerance: TF32 keeps 10 mantissa bits and the tensor core truncates the operands it reads, so a dot product carries ~1e-3 relative
 error; the bar here is 3e-3 relative L2 per tensor (the exact-fp32 mode holds 1e-5 on the same shapes, tests/test_gpu_train_ops.py)."""
@@ -108,7 +108,7 @@ def test_two_sources_then_transposed_conv_with_crop_tf32(eng):
 
 
 def test_wgrad_tc_against_simt_kernel_directly():
-    """aero_tapgemm_wgrad with precision 1 (tcgen05) against precision 0 (SIMT) on the same buffers: strided activations (a channel slice
+    """aero_tapgemm_wgrad with precision 1 (tensor cores) against precision 0 (SIMT) on the same buffers: strided activations (a channel slice
     of a wider tensor), un-padded time kernel (T_in != T) and a pixel count that leaves most split-K slices ragged."""
     lib = cabi.load()
     dev = torch.device("cuda")

@@ -69,10 +69,11 @@ def rel_l2(a, b):
     return float((a - b).norm() / b.norm().clamp_min(1e-30))
 
 
-def import_reference():
-    """Import the unmodified reference package (only possible where /root/reference exists)."""
+def import_reference(ref_root=None):
+    """Import the unmodified reference package from a checkout of slp-rl/aero (`ref_root`, default $AERO_REFERENCE);
+    None when there is none."""
     import importlib
-    ref_root = "/root/reference"
+    ref_root = os.path.abspath(ref_root or os.environ.get("AERO_REFERENCE") or "reference")
     if not os.path.isdir(ref_root):
         return None
     saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k == "src" or k.startswith("src.")}

@@ -169,7 +169,7 @@ def main():
     ap.add_argument("--no-stats", action="store_true")
     ap.add_argument("--out-f32", action="store_true")
     ap.add_argument("--in-f32", action="store_true")
-    ap.add_argument("--wgrad", action="store_true", help="time aero_tapgemm_wgrad of the shape (precision 0 = SIMT, 1 = tcgen05 TF32)")
+    ap.add_argument("--wgrad", action="store_true", help="time aero_tapgemm_wgrad of the shape (precision 0 = SIMT, 1 = tensor-core TF32)")
     args = ap.parse_args()
     torch.manual_seed(0)
     if args.shape.startswith("lstm"):

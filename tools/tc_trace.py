@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Pipeline timeline of the persistent tcgen05 tap-GEMM for one shape: builds a -DAERO_TC_TRACE twin of the library
-(clock64 stamps of CTA 0: producer / MMA issuer / epilogue events per tile) and prints per-tile intervals.
-    python tools/tc_trace.py enc0_rw"""
+"""Per-step timeline of the persistent LSTM recurrence for one shape: builds a -DAERO_TC_TRACE twin of the library
+(clock64 stamps of CTA 0: MMA warpgroup / cell-update events per step) and prints per-step intervals.
+    python tools/tc_trace.py lstm96"""
 import ctypes as C
 import glob
 import os
@@ -31,29 +31,15 @@ if __name__ == "__main__":
     sys.argv = [sys.argv[0], sys.argv[1], "--iters", "1"] + sys.argv[2:]
     kp.main()
     lib = cabi.load()
-    if sys.argv[1].startswith("lstm"):
-        buf = (C.c_longlong * (128 * 8))()
-        lib.aero_debug_lstm_trace.argtypes = [C.c_void_p]
-        assert lib.aero_debug_lstm_trace(buf) == 0
-        rows = [[buf[i * 8 + j] for j in range(8)] for i in range(128)]
-        names = ["mma:h_ready", "mma:commit", "upd:top", "upd:acc", "upd:act", "upd:h_stored", "upd:arrived"]
-        t0 = rows[1][0]
-        print("step " + " ".join(f"{n:>12s}" for n in names) + "   (cycles; update warp 0 lane 0)")
-        for i in range(1, int(os.environ.get("ROWS", 24))):
-            print(f"{i:4d} " + " ".join(f"{v - t0:12d}" if v else " " * 12 for v in rows[i][:7]))
-        print(f"steady state: {(rows[100][0] - rows[20][0]) / 80:.0f} cycles per step")
-        sys.exit(0)
-    buf = (C.c_longlong * (256 * 8))()
-    lib.aero_debug_tc_trace.argtypes = [C.c_void_p]
-    assert lib.aero_debug_tc_trace(buf) == 0
-    rows = [[buf[i * 8 + j] for j in range(8)] for i in range(256)]
-    rows = [r for r in rows if r[0]]
-    t0 = rows[0][0]
-    names = ["prod:start", "prod:issued", "mma:acc_free", "mma:data", "mma:commit", "epi:wait", "epi:acc", "epi:done"]
-    print("tile  " + " ".join(f"{n:>12s}" for n in names) + "   (cycles since first event; epi = warp with lane quarter 0 of the group)")
-    for i, r in enumerate(rows[:int(os.environ.get("ROWS", 40))]):
-        print(f"{i:4d}  " + " ".join(f"{v - t0:12d}" if v else " " * 12 for v in r))
-    if len(rows) > 8:
-        n = len(rows) - 4
-        per = (rows[n][7] - rows[4][7]) / (n - 4)
-        print(f"steady state: {per:.0f} cycles per tile (epilogue-done to epilogue-done)")
+    assert sys.argv[1].startswith("lstm"), "only the LSTM recurrence carries trace stamps"
+    buf = (C.c_longlong * (128 * 8))()
+    lib.aero_debug_lstm_trace.argtypes = [C.c_void_p]
+    assert lib.aero_debug_lstm_trace(buf) == 0
+    rows = [[buf[i * 8 + j] for j in range(8)] for i in range(128)]
+    names = ["mma:h_ready", "mma:commit", "upd:top", "upd:acc", "upd:act", "upd:h_stored", "upd:arrived"]
+    t0 = rows[1][0]
+    print("step " + " ".join(f"{n:>12s}" for n in names) + "   (cycles; update warp 0 lane 0)")
+    for i in range(1, int(os.environ.get("ROWS", 24))):
+        print(f"{i:4d} " + " ".join(f"{v - t0:12d}" if v else " " * 12 for v in rows[i][:7]))
+    print(f"steady state: {(rows[100][0] - rows[20][0]) / 80:.0f} cycles per step")
+    sys.exit(0)
