@@ -49,7 +49,7 @@ class EmuEngine(AeroEngine):
             v = torch.einsum("nk,bkm->bnm", w.reshape(N, -1)[:, :C1].double(), Av)
             if colscale is not None:
                 v = v * torch.as_strided(colscale.reshape(-1), (B, 1, T), (cs_s[0], 0, 1)).double()
-            torch.as_strided(out.reshape(-1), (B, N, T), (o_s[0], o_s[2], 1)).copy_(v.float())
+            torch.as_strided(out.reshape(-1), (B, N, T), (o_s[0], o_s[2], 1)).copy_(v)
             return out
         F_in = F_out if F_in is None else F_in
         T_in = T if T_in is None else T_in
@@ -75,7 +75,7 @@ class EmuEngine(AeroEngine):
             Wm = torch.as_strided(w.reshape(-1), (B, nslab, K, N), (w_sb, K * ldw, ldw, 1)).double()
         else:
             Wm = torch.as_strided(w.reshape(-1), (1, nslab, K, N), (0, K * ldw, ldw, 1)).double().expand(B, -1, -1, -1)
-        acc = torch.zeros(B, F_out, T, N, dtype=torch.float64)
+        acc = torch.zeros(B, F_out, T, N, dtype=torch.float64, device=A.device)     # runs wherever its inputs live
         for fo in range(F_out):
             for tap in range(ntaps):
                 if mode == cabi.TAPS_CONV:
@@ -107,9 +107,8 @@ class EmuEngine(AeroEngine):
             v = v + _view(residual, (B, F_out, T, n_out), (*r_s, 1)).double()
         if samp_affine is not None:
             v = v * samp_affine.double()[:, 0].view(B, 1, 1, 1) + samp_affine.double()[:, 1].view(B, 1, 1, 1)
-        vf = v.float()
-        _view(out, (B, F_out, T, n_out), (*o_s, 1)).copy_(vf)
-        vf = _view(out, (B, F_out, T, n_out), (*o_s, 1)).float()          # statistics describe the values as stored (FP16 raws)
+        _view(out, (B, F_out, T, n_out), (*o_s, 1)).copy_(v)              # one rounding, to the output's storage type
+        vf = _view(out, (B, F_out, T, n_out), (*o_s, 1))                   # statistics describe the values as stored (FP16 raws)
         if stats_mode == 1:
             g = vf.double().view(B, F_out * T, groups, n_out // groups)
             stats[:, 0] += g.sum((1, 3)).reshape(-1)

@@ -432,7 +432,8 @@ def test_freq_mix_small(engines, F, dt):
 
 
 def test_fp16_outputs_of_the_other_kernels(engines):
-    """norm_act / LSTM recurrence / attention writing FP16: the fp32 result of the same call, rounded once."""
+    """norm_act / attention writing FP16: the fp32 result of the same call, rounded once (the LSTM recurrence's FP16 output:
+    test_gpu_tc_scale.py)."""
     gpu, _ = engines
     B, F_in, T, Cc = 2, 6, 77, 48
     x = (rnd(B, F_in, T, Cc, seed=1) * 1.7 + 0.3).cuda()
