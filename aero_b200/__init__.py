@@ -2,11 +2,13 @@
 
 Public surface (mirrors the reference's ``src.models`` names):
   * ``Aero``                 -- drop-in for ``src.models.aero.Aero``
+  * ``Seanet``               -- drop-in for ``src.models.seanet.Seanet``
   * ``spectro`` / ``ispectro`` -- drop-ins for ``src.models.spec``
   * ``load_experiment``      -- Hydra-less reader of ``conf/experiment/*.yaml``
 """
 from .model import Aero, AeroGeometry  # noqa: F401
-from .config import load_experiment, aero_kwargs  # noqa: F401
+from .config import load_experiment, aero_kwargs, seanet_kwargs  # noqa: F401
+from .seanet import Seanet  # noqa: F401
 
 
 def spectro(x, n_fft=512, hop_length=None, pad=0, win_length=None):

@@ -61,11 +61,16 @@ class AttnParams(C.Structure):
     _fields_ = [("rows", i32), ("T", i32), ("H", i32), ("heads", i32), ("ndecay", i32), ("ld", i32), ("flags", i32)]
 
 
+class ResampleParams(C.Structure):
+    _fields_ = [("B", i32), ("C", i32), ("L_in", i32), ("orig", i32), ("up", i32), ("width", i32), ("taps", i32),
+                ("L_hr", i32), ("L_valid", i32), ("halo", i32), ("fill", i32), ("normalize", i32), ("floor_", f32)]
+
+
 ABI_VERSION = 3
 TAPS_CONV, TAPS_CONVT, TAPS_MIX = 0, 1, 2
-ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
+ACT_NONE, ACT_GELU, ACT_RELU, ACT_LEAKY, ACT_TANH = 0, 1, 2, 3, 4
 TG_ROUND_TF32, TG_A_F16, TG_OUT_F16, TG_REVERSE = 1, 2, 4, 8      # storage-type flags (AERO_TG_*)
-NA_NONE, NA_GELU, NA_GLU, NA_SNAKE, NA_GLU_SCALE_RES, NA_RELU, NA_LEAKY = 0, 1, 2, 3, 4, 5, 6
+NA_NONE, NA_GELU, NA_GLU, NA_SNAKE, NA_GLU_SCALE_RES, NA_RELU, NA_LEAKY, NA_TANH = 0, 1, 2, 3, 4, 5, 6, 7
 NA_NO_NORM = 16
 STFT_ZERO_PAD, STFT_ADJ_SCALE, ISTFT_RAW = 1, 2, 1
 
@@ -113,6 +118,12 @@ SYMBOLS = {
     "aero_lstm_fold": (C.c_int, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "aero_local_attn_train_fwd": (C.c_int, [vp, vp, vp, C.POINTER(AttnParams), vp]),
     "aero_local_attn_bwd": (C.c_int, [vp] * 5 + [C.POINTER(AttnParams), vp]),
+    # SEANet generator
+    "aero_seanet_input_fwd": (C.c_int, [vp, vp, vp, vp, C.POINTER(ResampleParams), vp]),
+    "aero_reflect_act_fwd": (C.c_int, [vp, vp, i32, i32, i32, i64, i64, i32, i32, i32, vp]),
+    "aero_reflect_act_bwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i64, i64, i32, i32, vp]),
+    "aero_seanet_output_fwd": (C.c_int, [vp, vp, vp, vp, i32, i64, vp]),
+    "aero_seanet_output_bwd": (C.c_int, [vp, vp, vp, vp, i32, i64, vp]),
 }
 
 

@@ -54,3 +54,9 @@ def aero_kwargs(name, conf_dir=None, **overrides):
     """kwargs for ``Aero(**...)`` from an experiment file."""
     exp = load_experiment(name, conf_dir, **overrides)
     return dict(exp["aero"])
+
+
+def seanet_kwargs(name, conf_dir=None, **overrides):
+    """kwargs for ``Seanet(**...)`` from an experiment file."""
+    exp = load_experiment(name, conf_dir, **overrides)
+    return dict(exp["seanet"])

@@ -24,6 +24,7 @@ __device__ __forceinline__ float gelu_exact(float x) {
     return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
+__device__ __forceinline__ float leaky_f(float x) { return x > 0.f ? x : 0.2f * x; }   // nn.LeakyReLU(0.2)
 
 // Round to TF32 (10-bit mantissa), nearest with ties away from zero -- the result of cvt.rna.tf32.f32 for every finite input,
 // in two integer instructions (ptxas expands the cvt into ~5 with Inf/NaN special-casing; Inf and NaN also survive this form:

@@ -1,0 +1,208 @@
+// SEANet input stage (reference src/models/seanet.py:158-168) and the reflection-halo pass that feeds its reflect-padded
+// convolutions (seanet.py:14-16,57-66,106-118).  See include/aero_b200.h for the contracts.
+#include "common.cuh"
+
+namespace aero {
+
+constexpr int kStatThreads = 256;
+
+// one CTA per clip: std of the channel mean (unbiased, two passes in fp64) -> affine[b] = {std, 0}
+__global__ void __launch_bounds__(kStatThreads) seanet_std_kernel(const float* __restrict__ x, float* __restrict__ affine,
+                                                                  const aero_resample_params p) {
+    __shared__ double red[kStatThreads / 32];
+    __shared__ double mean_s;
+    const int b = blockIdx.x;
+    const float* xb = x + (int64_t)b * p.C * p.L_in;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    auto mono = [&](int i) {
+        float s = 0.f;
+        for (int c = 0; c < p.C; ++c) s += xb[(int64_t)c * p.L_in + i];
+        return s / (float)p.C;
+    };
+    auto block_sum = [&](double v) {
+        v = warp_sum(v);
+        if (lane == 0) red[warp] = v;
+        __syncthreads();
+        double t = 0.0;
+        if (threadIdx.x == 0)
+            for (int w = 0; w < kStatThreads / 32; ++w) t += red[w];
+        __syncthreads();
+        return t;                                        // valid in thread 0
+    };
+    double s = 0.0;
+    for (int i = threadIdx.x; i < p.L_in; i += kStatThreads) s += mono(i);
+    s = block_sum(s);
+    if (threadIdx.x == 0) mean_s = s / p.L_in;
+    __syncthreads();
+    const double mean = mean_s;
+    double q = 0.0;
+    for (int i = threadIdx.x; i < p.L_in; i += kStatThreads) {
+        const double d = (double)mono(i) - mean;
+        q += d * d;
+    }
+    q = block_sum(q);
+    if (threadIdx.x == 0) {
+        affine[2 * b] = p.normalize ? (float)sqrt(q / (p.L_in - 1)) : 1.f;
+        affine[2 * b + 1] = 0.f;
+    }
+}
+
+// one thread per written (clip, frame, channel): normalise, polyphase filter, zero pad, reflect into the halo
+__global__ void __launch_bounds__(256) seanet_resample_kernel(const float* __restrict__ x, const float* __restrict__ filt,
+                                                              const float* __restrict__ affine, float* __restrict__ x0,
+                                                              const aero_resample_params p) {
+    const int span = p.L_valid + 2 * p.fill;
+    const int64_t n = (int64_t)p.B * span * p.C;
+    const int64_t rows = (int64_t)p.L_valid + 2 * p.halo;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % p.C);
+        const int64_t r = i / p.C;
+        const int u = (int)(r % span) - p.fill;
+        const int b = (int)(r / span);
+        int t = u < 0 ? -u : u;
+        if (t >= p.L_valid) t = 2 * (p.L_valid - 1) - t;
+        float v = 0.f;
+        if (t < p.L_hr) {
+            const float den = p.normalize ? p.floor_ + affine[2 * b] : 1.f;
+            const float* xs = x + ((int64_t)b * p.C + c) * p.L_in;
+            if (p.up == 0) {
+                v = xs[t] / den;
+            } else {
+                const int ph = t % p.up, s0 = (t / p.up) * p.orig - p.width;
+                const float* f = filt + (int64_t)ph * p.taps;
+                for (int k = 0; k < p.taps; ++k) {
+                    const int j = s0 + k;
+                    if (j >= 0 && j < p.L_in) v = fmaf(f[k], xs[j] / den, v);
+                }
+            }
+        }
+        x0[((int64_t)b * rows + p.halo + u) * p.C + c] = v;
+    }
+}
+
+template <typename TI, typename TO>
+__global__ void __launch_bounds__(256) reflect_act_kernel(const TI* __restrict__ x, TO* __restrict__ y, int B, int T, int C,
+                                                          int64_t x_sb, int64_t y_sb, int halo, int act, bool rnd) {
+    const int span = T + 2 * halo, cq = C / 4;
+    const int64_t n = (int64_t)B * span * cq;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % cq) * 4;
+        const int64_t r = i / cq;
+        const int u = (int)(r % span) - halo;
+        const int b = (int)(r / span);
+        int t = u < 0 ? -u : u;
+        if (t >= T) t = 2 * (T - 1) - t;
+        float4 v = ld4(x + (int64_t)b * x_sb + (int64_t)t * C + c);
+        if (act == AERO_ACT_LEAKY) {
+            v.x = v.x > 0.f ? v.x : 0.2f * v.x; v.y = v.y > 0.f ? v.y : 0.2f * v.y;
+            v.z = v.z > 0.f ? v.z : 0.2f * v.z; v.w = v.w > 0.f ? v.w : 0.2f * v.w;
+        }
+        if (rnd) { v.x = round_tf32_rna(v.x); v.y = round_tf32_rna(v.y); v.z = round_tf32_rna(v.z); v.w = round_tf32_rna(v.w); }
+        st4(y + (int64_t)b * y_sb + (int64_t)u * C + c, v);
+    }
+}
+
+__global__ void __launch_bounds__(256) reflect_act_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                                                              float* __restrict__ dx, int B, int T, int C, int64_t x_sb, int64_t dy_sb,
+                                                              int halo, int act) {
+    const int64_t n = (int64_t)B * T * C;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i % C);
+        const int64_t r = i / C;
+        const int t = (int)(r % T), b = (int)(r / T);
+        const float* d = dy + (int64_t)b * dy_sb + c;
+        float g = d[(int64_t)t * C];
+        if (t >= 1 && t <= halo) g += d[-(int64_t)t * C];                       // mirrored before frame 0
+        const int u = 2 * (T - 1) - t;                                           // mirrored after frame T-1
+        if (u >= T && u < T + halo) g += d[(int64_t)u * C];
+        if (act == AERO_ACT_LEAKY && !(x[(int64_t)b * x_sb + (int64_t)t * C + c] > 0.f)) g *= 0.2f;
+        dx[i] = g;
+    }
+}
+
+__global__ void __launch_bounds__(256) seanet_output_kernel(const float* __restrict__ v, const float* __restrict__ x0,
+                                                            const float* __restrict__ affine, const float* __restrict__ dy,
+                                                            float* __restrict__ out, int B, int64_t per_clip, bool bwd) {
+    const int64_t n = (int64_t)B * per_clip;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float s = affine[2 * (i / per_clip)];
+        const float t = tanhf(v[i]);
+        out[i] = bwd ? dy[i] * s * (1.f - t * t) : s * (t + x0[i]);
+    }
+}
+
+static int grid_for(int64_t n) {
+    const int64_t blocks = (n + 255) / 256;
+    return (int)(blocks < 132 * 16 ? (blocks < 1 ? 1 : blocks) : 132 * 16);
+}
+
+}  // namespace aero
+
+extern "C" int aero_seanet_input_fwd(const float* x, const float* filt, float* affine, float* x0, const aero_resample_params* pp,
+                                     aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(x && affine && x0 && pp, "aero_seanet_input_fwd: null argument");
+    const aero_resample_params& p = *pp;
+    AERO_REQUIRE(p.B >= 1 && p.C >= 1 && p.L_in >= 2, "aero_seanet_input_fwd: bad sizes (B=%d C=%d L_in=%d)", p.B, p.C, p.L_in);
+    AERO_REQUIRE(p.up >= 0 && (p.up == 0 || (filt && p.orig >= 1 && p.taps >= 1 && p.width >= 0)),
+                 "aero_seanet_input_fwd: bad filter (up=%d orig=%d taps=%d)", p.up, p.orig, p.taps);
+    AERO_REQUIRE(p.up != 0 || p.L_hr == p.L_in, "aero_seanet_input_fwd: without resampling L_hr must equal L_in");
+    AERO_REQUIRE(p.L_hr >= 1 && p.L_valid >= p.L_hr && p.fill >= 0 && p.fill <= p.halo && p.fill < p.L_valid,
+                 "aero_seanet_input_fwd: bad lengths (L_hr=%d L_valid=%d halo=%d fill=%d)", p.L_hr, p.L_valid, p.halo, p.fill);
+    cudaStream_t st = (cudaStream_t)stream;
+    seanet_std_kernel<<<p.B, kStatThreads, 0, st>>>(x, affine, p);
+    int rc = check_launch("aero_seanet_input_fwd(std)");
+    if (rc != AERO_OK) return rc;
+    seanet_resample_kernel<<<grid_for((int64_t)p.B * (p.L_valid + 2 * p.fill) * p.C), 256, 0, st>>>(x, filt, affine, x0, p);
+    return check_launch("aero_seanet_input_fwd(resample)");
+}
+
+extern "C" int aero_reflect_act_fwd(const void* x, void* y, int32_t B, int32_t T, int32_t C, int64_t x_sb, int64_t y_sb,
+                                    int32_t halo, int32_t act, int32_t flags, aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(x && y, "aero_reflect_act_fwd: null argument");
+    AERO_REQUIRE(B >= 1 && T >= 1 && C >= 4 && C % 4 == 0 && halo >= 0 && halo < T,
+                 "aero_reflect_act_fwd: bad sizes (B=%d T=%d C=%d halo=%d)", B, T, C, halo);
+    AERO_REQUIRE(act == AERO_ACT_NONE || act == AERO_ACT_LEAKY, "aero_reflect_act_fwd: act=%d", act);
+    const bool a16 = flags & AERO_TG_A_F16, o16 = flags & AERO_TG_OUT_F16, rnd = (flags & AERO_TG_ROUND_TF32) && !o16;
+    AERO_REQUIRE(!a16 || o16, "aero_reflect_act_fwd: FP16 input needs FP16 output");
+    const int g = grid_for((int64_t)B * (T + 2 * halo) * (C / 4));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (a16)
+        reflect_act_kernel<__half, __half><<<g, 256, 0, st>>>(static_cast<const __half*>(x), static_cast<__half*>(y), B, T, C, x_sb,
+                                                              y_sb, halo, act, false);
+    else if (o16)
+        reflect_act_kernel<float, __half><<<g, 256, 0, st>>>(static_cast<const float*>(x), static_cast<__half*>(y), B, T, C, x_sb,
+                                                             y_sb, halo, act, false);
+    else
+        reflect_act_kernel<float, float><<<g, 256, 0, st>>>(static_cast<const float*>(x), static_cast<float*>(y), B, T, C, x_sb,
+                                                            y_sb, halo, act, rnd);
+    return check_launch("aero_reflect_act_fwd");
+}
+
+extern "C" int aero_reflect_act_bwd(const float* x, const float* dy, float* dx, int32_t B, int32_t T, int32_t C, int64_t x_sb, int64_t dy_sb,
+                                    int32_t halo, int32_t act, aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(dy && dx && (x || act == AERO_ACT_NONE), "aero_reflect_act_bwd: null argument");
+    AERO_REQUIRE(B >= 1 && T >= 1 && C >= 1 && halo >= 0 && halo < T, "aero_reflect_act_bwd: bad sizes (B=%d T=%d C=%d halo=%d)", B, T, C,
+                 halo);
+    AERO_REQUIRE(act == AERO_ACT_NONE || act == AERO_ACT_LEAKY, "aero_reflect_act_bwd: act=%d", act);
+    reflect_act_bwd_kernel<<<grid_for((int64_t)B * T * C), 256, 0, (cudaStream_t)stream>>>(x, dy, dx, B, T, C, x_sb, dy_sb, halo, act);
+    return check_launch("aero_reflect_act_bwd");
+}
+
+extern "C" int aero_seanet_output_fwd(const float* v, const float* x0, const float* affine, float* y, int32_t B, int64_t per_clip,
+                                      aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(v && x0 && affine && y && B >= 1 && per_clip >= 1, "aero_seanet_output_fwd: bad arguments");
+    seanet_output_kernel<<<grid_for((int64_t)B * per_clip), 256, 0, (cudaStream_t)stream>>>(v, x0, affine, nullptr, y, B, per_clip, false);
+    return check_launch("aero_seanet_output_fwd");
+}
+
+extern "C" int aero_seanet_output_bwd(const float* v, const float* affine, const float* dy, float* dv, int32_t B, int64_t per_clip,
+                                      aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(v && affine && dy && dv && B >= 1 && per_clip >= 1, "aero_seanet_output_bwd: bad arguments");
+    seanet_output_kernel<<<grid_for((int64_t)B * per_clip), 256, 0, (cudaStream_t)stream>>>(v, nullptr, affine, dy, dv, B, per_clip, true);
+    return check_launch("aero_seanet_output_bwd");
+}

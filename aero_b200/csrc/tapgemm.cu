@@ -26,6 +26,7 @@ extern "C" int aero_tapgemm_fwd(const void* a1, const void* a2, const void* w, c
         set_error("aero_tapgemm_fwd: mode=%d", p.mode);
         return AERO_ERR_INVALID;
     }
+    AERO_REQUIRE(p.act >= AERO_ACT_NONE && p.act <= AERO_ACT_TANH, "aero_tapgemm_fwd: act=%d", p.act);
     AERO_REQUIRE(!p.glu || p.N % 2 == 0, "aero_tapgemm_fwd: GLU needs even N");
     const int Nout = p.glu ? p.N / 2 : p.N;
     if (p.stats_mode) {

@@ -149,6 +149,8 @@ __global__ void __launch_bounds__((BM / TM) * (BN / TN)) tapgemm_simt_kernel(con
                 if (g.colscale) x *= g.colscale[(int64_t)b * p.cs_sb + (int64_t)t * p.cs_st + n];
                 if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
                 else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
+                else if (p.act == AERO_ACT_LEAKY) x = leaky_f(x);
+                else if (p.act == AERO_ACT_TANH) x = tanhf(x);
             }
             v[j] = x;
         }
@@ -288,6 +290,8 @@ __global__ void __launch_bounds__(256) tapgemm_thin_n_kernel(const TapGemmArgs g
                 float x = acc[n] + (g.bias ? g.bias[n] : 0.f);
                 if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
                 else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
+                else if (p.act == AERO_ACT_LEAKY) x = leaky_f(x);
+                else if (p.act == AERO_ACT_TANH) x = tanhf(x);
                 if (rp) x += ldf(rp + n);
                 x = x * sa + sb;
                 if ((p.flags & 1) && sizeof(TO) == 4) x = round_tf32_rna(x);
@@ -362,6 +366,8 @@ __global__ void __launch_bounds__(256) tapgemm_thin_n_warp_kernel(const TapGemmA
                 float x = acc[n] + (g.bias ? g.bias[n] : 0.f);
                 if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
                 else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
+                else if (p.act == AERO_ACT_LEAKY) x = leaky_f(x);
+                else if (p.act == AERO_ACT_TANH) x = tanhf(x);
                 if (rp) x += ldf(rp + n);
                 x = x * sa + sb;
                 if ((p.flags & 1) && sizeof(TO) == 4) x = round_tf32_rna(x);
@@ -403,6 +409,8 @@ __global__ void __launch_bounds__(256) tapgemm_thin_k_kernel(const TapGemmArgs g
         }
         if (p.act == AERO_ACT_GELU) { acc.x = gelu_exact(acc.x); acc.y = gelu_exact(acc.y); acc.z = gelu_exact(acc.z); acc.w = gelu_exact(acc.w); }
         else if (p.act == AERO_ACT_RELU) { acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f); }
+        else if (p.act == AERO_ACT_LEAKY) { acc.x = leaky_f(acc.x); acc.y = leaky_f(acc.y); acc.z = leaky_f(acc.z); acc.w = leaky_f(acc.w); }
+        else if (p.act == AERO_ACT_TANH) { acc.x = tanhf(acc.x); acc.y = tanhf(acc.y); acc.z = tanhf(acc.z); acc.w = tanhf(acc.w); }
         if (rnd) { acc.x = round_tf32_rna(acc.x); acc.y = round_tf32_rna(acc.y); acc.z = round_tf32_rna(acc.z); acc.w = round_tf32_rna(acc.w); }
         st4(static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + (int64_t)fo * p.o_sf + (int64_t)t * p.o_st + n, acc);
     }
@@ -460,6 +468,8 @@ __global__ void __launch_bounds__(256) tapgemm_thin_convt_kernel(const TapGemmAr
                 float x = acc[v] + (g.bias ? g.bias[n] : 0.f);
                 if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
                 else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
+                else if (p.act == AERO_ACT_LEAKY) x = leaky_f(x);
+                else if (p.act == AERO_ACT_TANH) x = tanhf(x);
                 x = x * sa + sb;
                 if ((p.flags & 1) && sizeof(TO) == 4) x = round_tf32_rna(x);
                 stf(static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + (int64_t)fo * p.o_sf + (int64_t)t * p.o_st + n, x);

@@ -115,6 +115,9 @@ bool tapgemm_tc_eligible(const aero_tapgemm_params& p) {
         return p.w_sb == 0 && p.C1 % q == 0 && p.C2 == 0 && p.a1_st % q == 0 && p.a1_sb % q == 0 && p.N >= 8 &&
                p.stats_mode == 0 && !p.glu && p.F_out == 1 && p.F_in == 1 && tc_stages(p.N, pick_bn(p.N)) >= 2;
     if (p.w_sb != 0) return false;                                   // activations-as-weights (FTB frequency mix)
+    if (p.act == AERO_ACT_TANH) return false;                        // tanh is built for the SIMT kernels only (SEANet's thin layers)
+    if (p.act == AERO_ACT_LEAKY && (p.stats_mode != 0 || p.r_sb != 0 || p.r_sf != 0 || p.r_st != 0))
+        return false;                                                // LeakyReLU: plain epilogue only (no residual, no statistics)
     if (tc_stages(p.N, pick_bn(p.N)) < 2) return false;              // the bias of that many columns leaves no room for a pipeline
     if (p.N < 8) return false;                                       // thin outputs stay on the SIMT path
     const int K = p.C1 + p.C2;
@@ -210,7 +213,8 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
     }
     if (kn.stages >= 2 && kn.stages < kStages) kStages = kn.stages;
     const size_t smem = (size_t)kStages * stage_bytes + fixed;
-    const int amode = p.glu ? 3 : p.act;                 // the engine never combines GLU with an activation
+    // epilogue template mode: 0-2 = act, 3 = GLU, 4 = AERO_ACT_LEAKY (the engine never combines GLU with an activation)
+    const int amode = p.glu ? 3 : (p.act == AERO_ACT_LEAKY ? 4 : p.act);
     if (p.glu && p.act != AERO_ACT_NONE) { set_error("aero_tapgemm_fwd(wgmma): GLU with an activation is not supported"); return AERO_ERR_UNSUPPORTED; }
     const bool res = g.residual != nullptr, stats = p.stats_mode != 0;
     const KernelFn kern = BN == 32 ? tapgemm_tc_kernels_bn32(f16a, f16o, amode, res, stats)

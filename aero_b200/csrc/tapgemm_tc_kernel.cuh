@@ -85,7 +85,7 @@ __device__ __forceinline__ TileCoord tile_coord(const TapGemmArgs& g, int tile, 
     return c;
 }
 
-// Coalesced epilogue, specialised at compile time (AMODE: 0 none, 1 GELU, 2 ReLU, 3 GLU; RES: residual add; STATS).
+// Coalesced epilogue, specialised at compile time (AMODE: 0 none, 1 GELU, 2 ReLU, 3 GLU, 4 LeakyReLU(0.2); RES: residual add; STATS).
 // Stage A: this thread's 16 accumulator columns of its row -> bias -> activation / GLU -> row `lane` of the per-warp
 // staging tile.  Stage B: the warp walks the tile so that consecutive lanes hold consecutive float4s of one output row
 // (residual loads and stores are whole 32-byte sectors of one row), adds the row-wise terms, rounds, accumulates statistics.
@@ -103,6 +103,7 @@ __device__ __forceinline__ void epilogue_stage_a(const uint32_t (&r)[16], uint32
         for (int u = 0; u < 4; ++u) {
             if (AMODE == 1) v[u] = gelu_exact(v[u]);
             else if (AMODE == 2) v[u] = fmaxf(v[u], 0.f);
+            else if (AMODE == 4) v[u] = leaky_f(v[u]);
         }
         if (AMODE == 3) {
             sts64(stg_row + (j / 2) * 4, v[0] * sigmoid_f(v[1]), v[2] * sigmoid_f(v[3]));
@@ -250,7 +251,8 @@ __device__ __forceinline__ void epilogue_direct(TcShared* sh, const TapGemmArgs&
             for (int j = 0; j < 8; ++j) o[j] = v[2 * j] * sigmoid_f(v[2 * j + 1]);
         } else {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) o[j] = (AMODE == 1) ? gelu_exact(v[j]) : (AMODE == 2) ? fmaxf(v[j], 0.f) : v[j];
+            for (int j = 0; j < 16; ++j)
+                o[j] = (AMODE == 1) ? gelu_exact(v[j]) : (AMODE == 2) ? fmaxf(v[j], 0.f) : (AMODE == 4) ? leaky_f(v[j]) : v[j];
         }
         const int no0 = (AMODE == 3) ? nb >> 1 : nb;
         const int n_ok = min(CNT, Nout - no0);           // valid output columns of this chunk (a multiple of 4; 8 for FP16: host check)
@@ -544,6 +546,7 @@ tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_consta
                             if (csp) x *= csp[n];
                             if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
                             else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
+                            else if (AMODE == 4) x = leaky_f(x);
                         }
                         v[j] = x;
                     }
@@ -633,6 +636,7 @@ tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_consta
 template <int BN, bool F16A, bool F16O>
 static KernelFn pick_kernel(int amode, bool res, bool stats) {
 #define AERO_TC_K(A, R, S) tapgemm_tc_kernel<BN, A, R, S, F16A, F16O>
+    if (amode == 4) return (res || stats) ? nullptr : AERO_TC_K(4, false, false);   // LeakyReLU (SEANet): plain epilogue only
     if constexpr (!F16A && !F16O) {
         static const KernelFn table[4][2][2] = {
             {{AERO_TC_K(0, false, false), AERO_TC_K(0, false, true)}, {AERO_TC_K(0, true, false), AERO_TC_K(0, true, true)}},

@@ -573,6 +573,7 @@ __device__ __forceinline__ float na_act(int op, float g, float al) {
     if (op == AERO_NA_GELU) return gelu_exact(g);
     if (op == AERO_NA_RELU) return fmaxf(g, 0.f);
     if (op == AERO_NA_LEAKY) return g > 0.f ? g : 0.2f * g;
+    if (op == AERO_NA_TANH) return tanhf(g);
     if (op == AERO_NA_SNAKE) { const float sn = sinf(g * al); return g + sn * sn / al; }
     return g;
 }
@@ -583,6 +584,7 @@ __device__ __forceinline__ float na_dact(int op, float g, float al) {
     }
     if (op == AERO_NA_RELU) return g > 0.f ? 1.f : 0.f;
     if (op == AERO_NA_LEAKY) return g > 0.f ? 1.f : 0.2f;
+    if (op == AERO_NA_TANH) { const float t = tanhf(g); return 1.f - t * t; }
     if (op == AERO_NA_SNAKE) { return 1.0f + sinf(2.0f * g * al); }          // 1 + 2 sin(ag) cos(ag)
     return 1.f;
 }
@@ -1081,6 +1083,7 @@ extern "C" int aero_norm_act_train_fwd(const float* x, const double* stats, cons
         case AERO_NA_GLU_SCALE_RES: AERO_NAT(AERO_NA_GLU_SCALE_RES); break;
         case AERO_NA_RELU: AERO_NAT(AERO_NA_RELU); break;
         case AERO_NA_LEAKY: AERO_NAT(AERO_NA_LEAKY); break;
+        case AERO_NA_TANH: AERO_NAT(AERO_NA_TANH); break;
         default: set_error("aero_norm_act_train_fwd: op=%d", p->op); return AERO_ERR_INVALID;
     }
 #undef AERO_NAT
@@ -1111,6 +1114,7 @@ extern "C" int aero_norm_act_train_bwd(const float* x, const double* stats, cons
         case AERO_NA_GLU_SCALE_RES: AERO_NAB(AERO_NA_GLU_SCALE_RES); break;
         case AERO_NA_RELU: AERO_NAB(AERO_NA_RELU); break;
         case AERO_NA_LEAKY: AERO_NAB(AERO_NA_LEAKY); break;
+        case AERO_NA_TANH: AERO_NAB(AERO_NA_TANH); break;
         default: set_error("aero_norm_act_train_bwd: op=%d", p->op); return AERO_ERR_INVALID;
     }
 #undef AERO_NAB

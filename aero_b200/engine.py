@@ -111,7 +111,7 @@ class AeroEngine:
     def _init_state(self, model, lib):
         """All engine state (also used by the test / tooling subclasses that replace the kernel wrappers)."""
         self.model = model
-        self.geom = model.geom
+        self.geom = getattr(model, "geom", None)     # AERO geometry (SeanetEngine's model has none)
         self.lib = lib
         self._packed = None
         self._packed_key = None
@@ -356,12 +356,15 @@ class AeroEngine:
             W[p + ".ct.w"] = pack_taps(sd[p + ".conv_tr.weight"][:, :, :, 0].permute(1, 0, 2))
             W[p + ".ct.b"] = sd[p + ".conv_tr.bias"].contiguous()
         out = {k: (v.to(dev) if v.dtype == torch.float16 else v.to(device=dev, dtype=torch.float32)) for k, v in W.items()}
-        # K-major TF32 twins of every tap-GEMM weight for the wgmma path: [taps, K, pad4(N)] -> [taps, pad4(N), K]
-        # ... and FP16 twins [taps, pad4(N), pad8(K)] for the f16 wgmma
         self._wk, self._wh, self._wname = {}, {}, {}
         for k in [k for k in out if k.endswith("ftbfc.w")]:
             out[k + "@k"] = tf32_round(out[k])          # [F', F] is already K-contiguous
             out[k + "@h"] = pack_kmajor_fp16(out[k].t()[None].contiguous())[0]
+        return self._add_tc_twins(out)
+
+    def _add_tc_twins(self, out):
+        """K-major TF32 twins of every tap-GEMM weight `*.w` ([taps, K, pad4(N)]) for the wgmma path: [taps, pad4(N), K],
+        and FP16 twins [taps, pad4(N), pad8(K)] for the f16 wgmma; registered so that _gemm finds them by pointer."""
         for k in [k for k in out if k.endswith(".w") and out[k].dim() == 3]:
             out[k + "@k"] = tf32_round(out[k].permute(0, 2, 1).contiguous())
             out[k + "@h"] = pack_kmajor_fp16(out[k])

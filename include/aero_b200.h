@@ -115,7 +115,7 @@ int aero_istft_fwd(const float* z, const float* window, float* y,
  * 206,209,292), nn.Linear (modules.py:29,296) and their cuDNN/cuBLAS kernels.
  *
  * Epilogue, in order:  v = acc + bias[n];  v *= colscale[b][t][n]  (FTB gate, modules.py:314);
- *   act (none | exact GELU | ReLU);
+ *   act (none | exact GELU | ReLU | LeakyReLU(0.2) | tanh);
  *   GLU over adjacent column pairs (2j, 2j+1) -> channel j  (weights are stored pair-interleaved);
  *   v += addend_fn[fo][n'] (frequency embedding, aero.py:475-480);
  *   v = residual[b][fo][t][n'] + v  ;  v = v * samp_affine[b][0] + samp_affine[b][1] (aero.py:497-498);
@@ -125,7 +125,9 @@ int aero_istft_fwd(const float* z, const float* window, float* y,
  * source is at  src + b*sb + f*sf + t*st + c.
  */
 enum { AERO_TAPS_CONV = 0, AERO_TAPS_CONVT = 1, AERO_TAPS_MIX = 2 };
-enum { AERO_ACT_NONE = 0, AERO_ACT_GELU = 1, AERO_ACT_RELU = 2 };
+enum { AERO_ACT_NONE = 0, AERO_ACT_GELU = 1, AERO_ACT_RELU = 2,
+       AERO_ACT_LEAKY = 3 /* LeakyReLU(0.2); wgmma path: without residual or statistics */,
+       AERO_ACT_TANH = 4 /* SIMT path only (aero_tapgemm_tc_eligible() is 0) */ };
 typedef struct {
     int32_t B, F_out, T, N;
     int32_t F_in, T_in;
@@ -184,7 +186,7 @@ int aero_sample_norm_fwd(const float* x, const double* stats, float* y, float* s
  *     AERO_NA_GLU_SCALE_RES y[c] = residual[c] + scale[c] * glu(g)[c].
  */
 enum { AERO_NA_NONE = 0, AERO_NA_GELU = 1, AERO_NA_GLU = 2, AERO_NA_SNAKE = 3, AERO_NA_GLU_SCALE_RES = 4,
-       AERO_NA_RELU = 5, AERO_NA_LEAKY = 6 /* LeakyReLU(0.2) */ /* 5, 6: training entry points only */ };
+       AERO_NA_RELU = 5, AERO_NA_LEAKY = 6 /* LeakyReLU(0.2) */, AERO_NA_TANH = 7 /* 5-7: training entry points only */ };
 enum { AERO_NA_NO_NORM = 16 };      /* aero_norm_act_params.flags, training entry points: skip the normalisation (activation only) */
 typedef struct {
     int32_t B, F_in, F_out, f_off, T, C;
@@ -415,6 +417,48 @@ int aero_tapgemm_wgrad_tc_eligible(const aero_tapgemm_params* p, const float* a1
  * gradient (1/world_size after a sum all-reduce). */
 int aero_adam_step(const void* chunk_table, int32_t n_chunks, float lr, float beta1, float beta2, float eps, int32_t step,
                    float grad_scale, aero_stream_t stream);
+
+/* ==========================================================================================
+ * SEANet generator (reference src/models/seanet.py), time domain, channels-last activations [B][frames][C].
+ * ========================================================================================== */
+
+/* Input stage (seanet.py:158-168): per clip, std = unbiased std over the L_in samples of the channel mean (fp64 sums; 1 when
+ * normalize == 0), x' = x / (floor + std); then the polyphase Hann-windowed sinc resampler the reference calls (`up` phases of
+ * `taps` fp32 coefficients filt[up][taps], input stride `orig`, left pad `width`; up == 0: no resampling, L_hr = L_in), then zero
+ * padding to L_valid frames.  x : [B][C][L_in] fp32.  x0 : fp32, element (b, u, c) at x0 + b*(L_valid + 2*halo)*C + (halo + u)*C + c;
+ * frames u in [-fill, L_valid + fill) are written, the ones outside [0, L_valid) by reflection (fill < L_valid, fill <= halo).
+ * affine[b] = {std, 0}: the output scaling of seanet.py:179 as a tap-GEMM samp_affine. */
+typedef struct {
+    int32_t B, C, L_in;
+    int32_t orig, up, width, taps;
+    int32_t L_hr, L_valid, halo, fill;
+    int32_t normalize;
+    float floor_;
+} aero_resample_params;
+int aero_seanet_input_fwd(const float* x, const float* filt, float* affine, float* x0, const aero_resample_params* p,
+                          aero_stream_t stream);
+
+/* Reflection halo + activation (nn.ReflectionPad1d after nn.LeakyReLU, seanet.py:14-16,58-59):
+ *   y(b, u, c) = act(x(b, r(u), c)),  u in [-halo, T + halo),  r(u) = |u| reflected at both ends (halo < T),
+ * x element (b, t, c) at x + b*x_sb + t*C + c, y element (b, u, c) at y + b*y_sb + u*C + c (y points at frame 0; the halo
+ * frames lie before and after it).  act: AERO_ACT_NONE or AERO_ACT_LEAKY.  flags: AERO_TG_A_F16 (x FP16), AERO_TG_OUT_F16
+ * (y FP16), AERO_TG_ROUND_TF32 (fp32 y rounded to TF32).  C % 4 == 0.  A consumer convolution at dilation d then reads frame
+ * -d as its first input frame with no zero padding. */
+int aero_reflect_act_fwd(const void* x, void* y, int32_t B, int32_t T, int32_t C, int64_t x_sb, int64_t y_sb, int32_t halo,
+                         int32_t act, int32_t flags, aero_stream_t stream);
+
+/* Training adjoint of aero_reflect_act_fwd (fp32):  dx(b, t, c) = act'(x(b, t, c)) * sum over u with r(u) = t of dy(b, u, c),
+ * u in [-halo, T + halo): the halo's gradient folded back onto the mirrored frames.  dy element (b, u, c) at dy + b*dy_sb + u*C + c
+ * (dy points at frame 0), dx [B][T][C] contiguous, x as in the forward (act' needs it; unused for AERO_ACT_NONE). */
+int aero_reflect_act_bwd(const float* x, const float* dy, float* dx, int32_t B, int32_t T, int32_t C, int64_t x_sb, int64_t dy_sb,
+                         int32_t halo, int32_t act, aero_stream_t stream);
+
+/* SEANet output (seanet.py:116-118,176,179), training form: y[b][i] = affine[b][0] * (tanh(v[b][i]) + x0[b][i]), i < per_clip;
+ * backward dv[b][i] = dy[b][i] * affine[b][0] * (1 - tanh(v[b][i])^2).  All fp32, contiguous per clip. */
+int aero_seanet_output_fwd(const float* v, const float* x0, const float* affine, float* y, int32_t B, int64_t per_clip,
+                           aero_stream_t stream);
+int aero_seanet_output_bwd(const float* v, const float* affine, const float* dy, float* dv, int32_t B, int64_t per_clip,
+                           aero_stream_t stream);
 
 #ifdef __cplusplus
 }
