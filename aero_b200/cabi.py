@@ -124,6 +124,11 @@ SYMBOLS = {
     "aero_reflect_act_bwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i64, i64, i32, i32, vp]),
     "aero_seanet_output_fwd": (C.c_int, [vp, vp, vp, vp, i32, i64, vp]),
     "aero_seanet_output_bwd": (C.c_int, [vp, vp, vp, vp, i32, i64, vp]),
+    # HiFi-GAN multi-period discriminator
+    "aero_mpd_fold_fwd": (C.c_int, [vp, vp] + [i32] * 6 + [vp]),
+    "aero_mpd_fold_bwd": (C.c_int, [vp, vp] + [i32] * 6 + [vp]),
+    "aero_mpd_repack_fwd": (C.c_int, [vp, vp] + [i32] * 6 + [f32, vp]),
+    "aero_mpd_repack_bwd": (C.c_int, [vp, vp, vp] + [i32] * 6 + [f32, vp]),
 }
 
 

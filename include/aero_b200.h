@@ -460,6 +460,31 @@ int aero_seanet_output_fwd(const float* v, const float* x0, const float* affine,
 int aero_seanet_output_bwd(const float* v, const float* affine, const float* dy, float* dv, int32_t B, int64_t per_clip,
                            aero_stream_t stream);
 
+/* ==========================================================================================
+ * HiFi-GAN multi-period discriminator (reference src/models/discriminators.py:89-147), fp32.  Each period's activations are one
+ * long channels-last sequence of B*period segments s = b*period + w; segment s holds frames h of column w of the [T/period, period]
+ * view at rows s*seg + halo + h, and zeros at every other row (see DESIGN.md, "Multi-period discriminator").
+ * ========================================================================================== */
+
+/* Period fold (discriminators.py:107-113): x [B][T] -> y [B*period][seg] with y[(b*period + w)*seg + halo + h] = xp[b][h*period + w],
+ * h < H = ceil(T / period), where xp is x reflect-padded on the right to H*period samples (H*period - T < T); every other element of y
+ * is written 0.  Backward: dx[b][t] = dy at the position of t + dy at the position of its mirror 2(T-1) - t when that lies in the
+ * padding (the gradient that reaches the generator). */
+int aero_mpd_fold_fwd(const float* x, float* y, int32_t B, int32_t T, int32_t period, int32_t H, int32_t seg, int32_t halo,
+                      aero_stream_t stream);
+int aero_mpd_fold_bwd(const float* dy, float* dx, int32_t B, int32_t T, int32_t period, int32_t H, int32_t seg, int32_t halo,
+                      aero_stream_t stream);
+
+/* Activation repack (LeakyReLU(slope) after each convolution, discriminators.py:116-118): x element (s, h, c) at
+ * x[(s*rows_in + h)*C + c], h < H (a convolution's output rows; rows H .. rows_in-1 of a segment are ignored) ->
+ * y[(s*seg + halo + h)*C + c] = leaky(x), every other element of y [S][seg][C] written 0, so that y is the next convolution's input.
+ * Backward: dx[(s*rows_in + r)*C + c] = dy[(s*seg + halo + r)*C + c] * leaky'(x) for r < H and 0 for r >= H (every element of dx
+ * written: rows no output frame owns carry no gradient into the weight and bias sums).  C % 4 == 0, pointers 16-byte aligned. */
+int aero_mpd_repack_fwd(const float* x, float* y, int32_t S, int32_t H, int32_t C, int32_t rows_in, int32_t seg, int32_t halo,
+                        float slope, aero_stream_t stream);
+int aero_mpd_repack_bwd(const float* x, const float* dy, float* dx, int32_t S, int32_t H, int32_t C, int32_t rows_in, int32_t seg,
+                        int32_t halo, float slope, aero_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
