@@ -66,6 +66,11 @@ class ResampleParams(C.Structure):
                 ("L_hr", i32), ("L_valid", i32), ("halo", i32), ("fill", i32), ("normalize", i32), ("floor_", f32)]
 
 
+class GanTerm(C.Structure):
+    _fields_ = [("x", vp), ("ref", vp), ("dx", vp), ("adv_scale", C.c_double), ("l1_scale", C.c_double),
+                ("n_seg", i32), ("seg", i32), ("halo", i32), ("H", i32), ("C", i32), ("adv", i32)]
+
+
 ABI_VERSION = 3
 TAPS_CONV, TAPS_CONVT, TAPS_MIX = 0, 1, 2
 ACT_NONE, ACT_GELU, ACT_RELU, ACT_LEAKY, ACT_TANH = 0, 1, 2, 3, 4
@@ -73,6 +78,8 @@ TG_ROUND_TF32, TG_A_F16, TG_OUT_F16, TG_REVERSE = 1, 2, 4, 8      # storage-type
 NA_NONE, NA_GELU, NA_GLU, NA_SNAKE, NA_GLU_SCALE_RES, NA_RELU, NA_LEAKY, NA_TANH = 0, 1, 2, 3, 4, 5, 6, 7
 NA_NO_NORM = 16
 STFT_ZERO_PAD, STFT_ADJ_SCALE, ISTFT_RAW = 1, 2, 1
+GAN_NONE, GAN_LSGAN_REAL, GAN_LSGAN_FAKE, GAN_LSGAN_GEN, GAN_HINGE_REAL, GAN_HINGE_FAKE, GAN_HINGE_GEN = 0, 1, 2, 3, 4, 5, 6
+GAN_FWD_BLOCKS = 128                                              # AERO_GAN_FWD_BLOCKS
 
 # every symbol include/aero_b200.h declares (tests/test_cabi.py checks the library exports them all)
 SYMBOLS = {
@@ -129,6 +136,9 @@ SYMBOLS = {
     "aero_mpd_fold_bwd": (C.c_int, [vp, vp] + [i32] * 6 + [vp]),
     "aero_mpd_repack_fwd": (C.c_int, [vp, vp] + [i32] * 6 + [f32, vp]),
     "aero_mpd_repack_bwd": (C.c_int, [vp, vp, vp] + [i32] * 6 + [f32, vp]),
+    # GAN loss terms
+    "aero_gan_loss_fwd": (C.c_int, [vp, i32, vp, vp, vp]),
+    "aero_gan_loss_bwd": (C.c_int, [vp, i32, vp]),
 }
 
 

@@ -112,12 +112,13 @@ class _DiscEngine(TrainEngine):
             dy = self.grad(y)
             if dy is None:
                 return
-            gw = torch.zeros_like(w)
-            self._check(lib.aero_gconv1d_wgrad(_ptr(x), _ptr(dy), _ptr(gw), *args, self._stream()))
-            w_back(gw)
-            gb = self._new(Cout, zero=True, dtype=torch.float64)
-            self._colsum(dy, gb, Cout, B * Tout, Cout)
-            self._add_f64(self.pgrad(prefix + ".bias"), gb)
+            if self.param_grads:
+                gw = torch.zeros_like(w)
+                self._check(lib.aero_gconv1d_wgrad(_ptr(x), _ptr(dy), _ptr(gw), *args, self._stream()))
+                w_back(gw)
+                gb = self._new(Cout, zero=True, dtype=torch.float64)
+                self._colsum(dy, gb, Cout, B * Tout, Cout)
+                self._add_f64(self.pgrad(prefix + ".bias"), gb)
             if id(x) not in self.no_grad:
                 dx = self._new(B * Tin * Cin)
                 self._check(lib.aero_gconv1d_dgrad(_ptr(dy), _ptr(w), _ptr(dx), *args, self._stream()))
@@ -157,11 +158,14 @@ class _DiscEngine(TrainEngine):
         return [y.view(B, To, c) for y, To, c in outs]
 
     @torch.no_grad()
-    def backward(self, grads):
+    def backward(self, grads, grad_sink=None, owned=False):
+        """grads: one gradient (or None) per layer output.  grad_sink(name) -> zeroed tensor to accumulate that parameter's gradient
+        into (else fresh tensors).  owned: the gradients are flat fp32 buffers the tape may take over and modify (no copy)."""
         self._sync_stream()
+        self._sink = grad_sink
         for (y, To, c), gy in zip(self._outs, grads):
             if gy is not None:
-                self.acc(y, gy.contiguous().float().reshape(-1).clone())
+                self.acc(y, gy if owned else gy.contiguous().float().reshape(-1).clone())
         for fn in reversed(self.tape):
             fn()
         gx = self.g.get(id(self._x_in))

@@ -264,11 +264,13 @@ class _MpdEngine(_DiscEngine):
         return outs
 
     @torch.no_grad()
-    def backward(self, grads):
+    def backward(self, grads, grad_sink=None, owned=False):
+        """As _DiscEngine.backward: one gradient (or None) per stored output of forward()."""
         self._sync_stream()
+        self._sink = grad_sink
         for t, g in zip(self._outs, grads):
             if g is not None:
-                self.acc(t, g.contiguous().float().reshape(-1).clone())
+                self.acc(t, g if owned else g.contiguous().float().reshape(-1).clone())
         ends = {end - 1: (name, start) for name, start, end in self._spans}
         open_ = {}
         for i in range(len(self.tape) - 1, -1, -1):

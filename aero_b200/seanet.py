@@ -553,6 +553,7 @@ class SeanetTrainEngine(TrainEngine):
         h = self.conv(xp, None, Cin, 0, None, "encoder.0.1.bias", _Conv(kt=7), B, 1, 1, Lv, c, w_override=self._wn("encoder.0.1"),
                       T_in=Lv + 6)
         h = self.norm_act(h, cabi.NA_TANH, B=B, F_in=1, T=Lv, C_=c, scope=1, no_norm=True)
+        self.marks.append((len(self.tape), "encoder.0"))
         skips = [h]
         for i in range(1, nlev + 1):
             T, r = lev[i - 1], m.ratios[nlev - i]
@@ -567,10 +568,13 @@ class SeanetTrainEngine(TrainEngine):
                           w_override=(wp, lambda g, back=back, r=r, k=w.shape[2], shp=wp.shape: back(superframe_conv_weight_adjoint(
                               g.reshape(shp), r, k).contiguous())))
             skips.append(y)
+            self.marks.append((len(self.tape), f"encoder.{i}"))
             c *= 2
         T = lev[nlev]
         z = self.k7(skips[-1], f"encoder.{nlev + 1}.2", B, T, c, m.latent_space_size)
+        self.marks.append((len(self.tape), f"encoder.{nlev + 1}"))
         d = self.k7(z, "decoder.0.2", B, T, m.latent_space_size, c, residual=skips[-1])
+        self.marks.append((len(self.tape), "decoder.0"))
         for j in range(1, nlev + 1):
             r, co = m.ratios[j - 1], c // 2
             key = f"decoder.{j}.1"
@@ -587,7 +591,9 @@ class SeanetTrainEngine(TrainEngine):
             for k in range(nres):
                 x = self.resblock(x, f"decoder.{j}.{2 + k}", B, T, c, 3 ** k, residual=skip if k == nres - 1 else None)
             d = x
+            self.marks.append((len(self.tape), f"decoder.{j}"))
         v = self.k7(d, f"decoder.{nlev + 1}.2", B, Lv, c, m.out_channels)
+        self.marks.append((len(self.tape), f"decoder.{nlev + 1}"))
         out = self._new(B * Lv * m.out_channels)
         n = Lv * m.out_channels
         self._check(self.lib.aero_seanet_output_fwd(_ptr(v), _ptr(x0), _ptr(self._affine), _ptr(out), B, n, self._stream()))
@@ -607,15 +613,24 @@ class SeanetTrainEngine(TrainEngine):
         return out.view(B, Lv, m.out_channels)[:, :target].permute(0, 2, 1).contiguous()
 
     @torch.no_grad()
-    def backward(self, d_out):
-        """d_out [B, C, target] -> {parameter name: gradient}."""
+    def backward(self, d_out, grad_sink=None, on_layer_done=None):
+        """d_out [B, C, target] -> {parameter name: gradient}.  grad_sink(name) -> zeroed tensor to accumulate that parameter's gradient
+        into (else fresh tensors); on_layer_done(tag) is called when every gradient of top-level module `tag` ("decoder.5", ...,
+        "decoder.0", "encoder.5", ..., "encoder.0") is final (as TrainEngine.backward)."""
         self._sync_stream()
+        self._sink = grad_sink
         B, Lv, Co = self._shape
         g = torch.zeros(B, Lv, Co, dtype=torch.float32, device=d_out.device)
         g[:, :self._target] = d_out.permute(0, 2, 1)
         self.acc(self._out, g.view(-1))
-        for fn in reversed(self.tape):
-            fn()
+        starts, prev = {}, 0
+        for end, tag in self.marks:                       # module `tag` owns tape[prev:end]; it is done once tape[prev] has run
+            starts[prev] = tag
+            prev = end
+        for i in range(len(self.tape) - 1, -1, -1):
+            self.tape[i]()
+            if on_layer_done is not None and i in starts:
+                on_layer_done(starts[i])
         pg = self.pg
         self._reset()
         return pg

@@ -44,6 +44,10 @@ _C1x1 = _Conv()
 
 
 class TrainEngine:
+    # False: the tape computes data gradients only -- the convolutions skip their weight-gradient GEMMs, bias column sums and
+    # derived-weight callbacks (the generator pass of aero_b200.trainer.GanTrainer, whose optimiser does not use them)
+    param_grads = True
+
     def __init__(self, model):
         self.model = model
         self.geom = model.geom
@@ -300,20 +304,21 @@ class TrainEngine:
                 dy = d2
             if residual is not None:
                 self.acc(residual, dy)
-            # ---- weight gradient, written in the parameter's own layout
-            direct = w_back is None and wslice is None
-            gw = self.pgrad(wname).view(w4.shape) if direct else torch.zeros_like(w4, memory_format=torch.contiguous_format)
-            sn, sk = (gw.stride(0), gw.stride(1)) if cv.kind == "conv" else (gw.stride(1), gw.stride(0))
-            pw = self._tg(**geo)
             halves = {} if self.precision == 3 else None          # dy is split once for the weight and the data gradient
-            self._wgrad_call(x1, x2, dy, gw, pw, sn, sk, 1, halves)
-            if w_back is not None:
-                w_back(gw)
-            elif wslice is not None:
-                full = self.pgrad(wname)
-                (full[:, wslice] if cv.kind == "conv" else full[wslice]).add_(gw.view(w.shape))
+            # ---- weight gradient, written in the parameter's own layout
+            if self.param_grads:
+                direct = w_back is None and wslice is None
+                gw = self.pgrad(wname).view(w4.shape) if direct else torch.zeros_like(w4, memory_format=torch.contiguous_format)
+                sn, sk = (gw.stride(0), gw.stride(1)) if cv.kind == "conv" else (gw.stride(1), gw.stride(0))
+                pw = self._tg(**geo)
+                self._wgrad_call(x1, x2, dy, gw, pw, sn, sk, 1, halves)
+                if w_back is not None:
+                    w_back(gw)
+                elif wslice is not None:
+                    full = self.pgrad(wname)
+                    (full[:, wslice] if cv.kind == "conv" else full[wslice]).add_(gw.view(w.shape))
             # ---- bias gradient: column sums over every output pixel
-            if bias is not None:
+            if bias is not None and self.param_grads:
                 gb = self._new(N, zero=True, dtype=torch.float64)
                 self._colsum(dy, gb, N, T, os_[2], n_outer=F_out, outer_s=os_[1], n_seg=B, seg_sx=os_[0], seg_so=0)
                 if b_back is not None:

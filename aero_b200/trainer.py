@@ -11,14 +11,20 @@
 * ``aero_adam_step`` (one launch) applies Adam to every parameter with the 1/world_size averaging folded in.
 
 The plain autograd route (``loss.backward(); optimizer.step()``, DDP-wrapped or not) keeps working -- this class is the fast path
-that ``bench.py --config train`` measures.
+that ``bench.py --config train`` measures.  The generator is ``aero_b200.Aero`` or ``aero_b200.Seanet``.
+
+``GanTrainer(generator, {name: discriminator, ...})`` runs the reference's full adversarial step against ``msd_melgan`` and / or
+``mpd`` (DESIGN.md, "The adversarial step"); ``GanTrainer(aero, Discriminator)`` keeps the original single-MelGAN step.
 """
 from __future__ import annotations
+
+from collections.abc import Mapping
 
 import torch
 import torch.distributed as dist
 
 from .optim import FusedAdam
+from .seanet import Seanet, SeanetTrainEngine
 from .train_engine import TrainEngine
 
 
@@ -38,12 +44,23 @@ def _backward_order(model):
     return sorted(names, key=key)
 
 
+def _seanet_backward_order(model):
+    """SEANet's parameter names in the order SeanetTrainEngine.backward completes them: the decoder's top-level modules from the last
+    (decoder.{n+1}, the output convolution) to decoder.0, then the encoder's from encoder.{n+1} (the latent projection) to encoder.0."""
+    names = [n for n, _ in model.named_parameters()]
+
+    def key(n):
+        head, idx = n.split(".")[0], int(n.split(".")[1])
+        return (0 if head == "decoder" else 1, -idx)
+    return sorted(names, key=key)
+
+
 class GeneratorTrainer:
     def __init__(self, model, lr=3e-4, betas=(0.9, 0.999), eps=1e-8, pieces=4):
         self.model = model
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.params = dict(model.named_parameters())
-        self.order = _backward_order(model)
+        self.order = _seanet_backward_order(model) if isinstance(model, Seanet) else _backward_order(model)
         dev = next(model.parameters()).device
         total = sum(self.params[n].numel() for n in self.order)
         self.flat = torch.zeros(total, device=dev)
@@ -81,6 +98,13 @@ class GeneratorTrainer:
 
     def zero_grad(self):
         self.flat.zero_()
+
+    def _engine(self):
+        return SeanetTrainEngine(self.model) if isinstance(self.model, Seanet) else TrainEngine(self.model)
+
+    def _forward(self, eng, lr_batch):
+        out = eng.forward(lr_batch)
+        return out[0] if isinstance(out, tuple) else out         # Aero's engine also returns the output spectrogram
 
     def backward(self, engine, d_wave):
         """Run the tape with parameter gradients accumulating into the flat buffer; all-reduce finished pieces while the rest
@@ -122,8 +146,8 @@ class GeneratorTrainer:
         model.train()
         self.zero_grad()
         with torch.cuda.device(lr_batch.device):
-            eng = TrainEngine(model)
-            wave, _ = eng.forward(lr_batch)
+            eng = self._engine()
+            wave = self._forward(eng, lr_batch)
             pr = wave.detach().requires_grad_(True)
             loss = loss_fn(pr)
             loss.backward()
@@ -133,13 +157,27 @@ class GeneratorTrainer:
 
 
 class GanTrainer(GeneratorTrainer):
-    """The reference's full step with ``adversarial: True`` (``conf/experiment/aero_*.yaml``, ``src/solver.py:292-342,475-520,602-612``):
-    generator loss = MR-STFT + hinge adversarial + 100 x feature matching against the MelGAN multi-scale discriminator, then the
-    discriminator's hinge loss on (detached estimate, target); both optimisers are fused Adams; under ``torch.distributed`` the
-    discriminator's gradients are summed in one flat NCCL all-reduce as well."""
+    """The reference's full step with ``adversarial: True`` (``src/solver.py:292-342,428-520,580-612``, ``train.py:83-95``).
 
-    def __init__(self, model, disc, lr=3e-4, betas=(0.9, 0.999), eps=1e-8, features_loss_lambda=100.0, n_layers=4, pieces=4):
+    ``GanTrainer(generator, discs, features_loss_lambda=100, only_features_loss=False, only_adversarial_loss=False)``: generator
+    ``Aero`` or ``Seanet``; discs ``{name: module}`` keyed and ordered like ``discriminator_models`` -- ``'msd_melgan'``
+    (``aero_b200.discriminator.Discriminator``) and / or ``'mpd'`` (``aero_b200.mpd.MultiPeriodDiscriminator``).  ``step`` drives the
+    engines directly (``aero_b200.gan``): per discriminator one joint forward over ``[hr, pr.detach()]`` whose backward writes
+    parameter gradients only, and one forward of ``pr`` whose backward computes the input gradient only.  One FusedAdam over all
+    discriminators' parameters in ``discriminator_models`` order (as ``train.py`` chains them); their gradients live in one flat
+    buffer, summed over NCCL once per step under ``torch.distributed``.
+
+    ``GanTrainer(aero, disc)`` with a single MelGAN ``Discriminator`` module is the original step: generator loss = MR-STFT + hinge
+    adversarial + 100 x feature matching, then the discriminator's hinge loss on (detached estimate, target), through autograd on the
+    discriminator (n_layers: its ``melgan_discriminator.n_layers``)."""
+
+    def __init__(self, model, disc, lr=3e-4, betas=(0.9, 0.999), eps=1e-8, features_loss_lambda=100.0, n_layers=4, pieces=4,
+                 only_features_loss=False, only_adversarial_loss=False):
         super().__init__(model, lr=lr, betas=betas, eps=eps, pieces=pieces)
+        if isinstance(disc, Mapping):
+            self._init_discs(disc, lr, betas, eps, features_loss_lambda, only_features_loss, only_adversarial_loss)
+            return
+        self.discs = None
         self.disc = disc
         self.lmbda, self.n_layers = features_loss_lambda, n_layers
         dps = list(disc.parameters())
@@ -149,6 +187,22 @@ class GanTrainer(GeneratorTrainer):
             p.grad = self.d_flat[off:off + p.numel()].view(p.shape)
             off += p.numel()
         self.d_opt = FusedAdam(dps, lr=lr, betas=betas, eps=eps)
+
+    def _init_discs(self, discs, lr, betas, eps, lmbda, only_features, only_adversarial):
+        from .gan import check_discriminators
+        self.discs = check_discriminators(discs)
+        self.disc = None
+        self.lmbda = float(lmbda)
+        self.only_features, self.only_adversarial = bool(only_features), bool(only_adversarial)
+        dps = [(name, n, p) for name, d in self.discs.items() for n, p in d.named_parameters()]
+        self.d_flat = torch.zeros(sum(p.numel() for _, _, p in dps), device=dps[0][2].device)
+        self.d_views, off = {}, 0
+        for name, n, p in dps:
+            v = self.d_flat[off:off + p.numel()].view(p.shape)
+            self.d_views[(name, n)] = v
+            p.grad = v
+            off += p.numel()
+        self.d_opt = FusedAdam([p for _, _, p in dps], lr=lr, betas=betas, eps=eps)
 
     def generator_losses(self, pr, hr, stft_loss):
         """reference solver.py:430-473,499-520"""
@@ -170,6 +224,12 @@ class GanTrainer(GeneratorTrainer):
         return sum(relu(1 + s[-1]).mean() for s in fake) + sum(relu(1 - s[-1]).mean() for s in real)
 
     def step(self, lr_batch, hr_batch, stft_loss):
+        """One optimisation step of both networks.  With a discriminator mapping: returns the reference's loss mapping
+        ``{'generator': {'stft', 'adversarial_melgan', 'features_melgan', 'adversarial_mpd', 'features_mpd'}, 'discriminator':
+        {'msd_melgan', 'mpd'}}`` (the keys that apply), values 0-dim device tensors, not synchronised.  stft_loss(pr, hr) -> (sc, mag),
+        e.g. aero_b200.losses.MultiResolutionSTFTLoss(); None leaves the MR-STFT term out."""
+        if self.discs is not None:
+            return self._step_discs(lr_batch, hr_batch, stft_loss)
         model = self.model
         model.train()
         self.zero_grad()
@@ -191,3 +251,47 @@ class GanTrainer(GeneratorTrainer):
                 self.allreduce_bytes += self.d_flat.numel() * 4
             self.d_opt.step(grad_scale=1.0 / self.world)
         return {k: v.detach() for k, v in g_losses.items()} | {"discriminator": d_loss.detach()}
+
+    def _step_discs(self, lr_batch, hr_batch, stft_loss):
+        from .gan import ADVERSARIES
+        model = self.model
+        model.train()
+        self.zero_grad()
+        self.d_flat.zero_()
+        g_losses, d_losses = {}, {}
+        with torch.cuda.device(lr_batch.device):
+            eng = self._engine()
+            wave = self._forward(eng, lr_batch)
+            if wave.shape != hr_batch.shape:
+                raise ValueError(f"generator output {tuple(wave.shape)} and target {tuple(hr_batch.shape)} differ in shape")
+            pr = wave.detach().requires_grad_(True)
+            hr = hr_batch.detach().float().contiguous()
+            roots, grads = [], []
+            if stft_loss is not None:
+                sc, mag = stft_loss(pr.squeeze(1), hr.squeeze(1))
+                g_losses["stft"] = sc + mag
+                roots.append(g_losses["stft"])
+                grads.append(None)
+            for name, d in self.discs.items():
+                adv = ADVERSARIES[name](d, lambda n, name=name: self.d_views[(name, n)], self.lmbda, not self.only_features,
+                                        not self.only_adversarial)
+                d_losses[name] = adv.discriminator_pass(hr, pr)
+                losses, r, g = adv.generator_pass(pr)
+                g_losses.update(losses)
+                roots += r
+                grads += g
+            main = torch.cuda.current_stream()
+            if self.world > 1:                 # the discriminators' all-reduce overlaps the generator's backward
+                self.comm_stream.wait_stream(main)
+                with torch.cuda.stream(self.comm_stream):
+                    dist.all_reduce(self.d_flat)
+                self.allreduce_bytes += self.d_flat.numel() * 4
+            if roots:
+                torch.autograd.backward(roots, grads)
+            if pr.grad is not None:
+                self.backward(eng, pr.grad)
+            elif self.world > 1:
+                main.wait_stream(self.comm_stream)
+            self.opt.step(grad_scale=1.0 / self.world)
+            self.d_opt.step(grad_scale=1.0 / self.world)
+        return {"generator": {k: v.detach() for k, v in g_losses.items()}, "discriminator": d_losses}

@@ -485,6 +485,46 @@ int aero_mpd_repack_fwd(const float* x, float* y, int32_t S, int32_t H, int32_t 
 int aero_mpd_repack_bwd(const float* x, const float* dy, float* dx, int32_t S, int32_t H, int32_t C, int32_t rows_in, int32_t seg,
                         int32_t halo, float slope, aero_stream_t stream);
 
+/* ==========================================================================================
+ * GAN loss terms (reference src/solver.py:475-520, src/models/discriminators.py:211-244) on the discriminators' own storage.
+ * A term is one feature map stored as n_seg segments of seg rows x C channels, channels-last: element (s, h, c) of the map sits at
+ * x[(s*seg + halo + h)*C + c], h < H (the owned rows); the other rows of a segment belong to no output.  This is the MPD segment
+ * layout and, with one segment per clip and halo 0, MelGAN's [B, T, C].  Its count is n = n_seg*H*C.
+ * ========================================================================================== */
+
+enum {
+    AERO_GAN_NONE = 0,
+    AERO_GAN_LSGAN_REAL = 1,   /* (1 - x)^2                        (discriminator, real clips)      */
+    AERO_GAN_LSGAN_FAKE = 2,   /* x^2                              (discriminator, generated clips) */
+    AERO_GAN_LSGAN_GEN = 3,    /* (1 - x)^2                        (generator)                      */
+    AERO_GAN_HINGE_REAL = 4,   /* relu(1 - x)                      (discriminator, real clips)      */
+    AERO_GAN_HINGE_FAKE = 5,   /* relu(1 + x)                      (discriminator, generated clips) */
+    AERO_GAN_HINGE_GEN = 6     /* relu(1 - x)                      (generator)                      */
+};
+
+#define AERO_GAN_FWD_BLOCKS 128   /* blocks per term of aero_gan_loss_fwd: its workspace holds n_terms * 2 * this many doubles */
+
+typedef struct {
+    const float* x;      /* the map                                                                      */
+    const float* ref;    /* L1 reference map of the same geometry (the real clips' features), or NULL    */
+    float* dx;           /* gradient storage of x, n_seg*seg*C floats (aero_gan_loss_bwd)                */
+    double adv_scale;    /* weight / count of the adversarial mean (0: no adversarial component)         */
+    double l1_scale;     /* weight / count of the L1 mean (0 or ref NULL: no L1 component)               */
+    int32_t n_seg, seg, halo, H, C;
+    int32_t adv;         /* AERO_GAN_*                                                                   */
+} aero_gan_term;
+
+/* Forward of n_terms terms (terms: a DEVICE table) in one call: out[2t] = adv_scale * sum adv(x), out[2t + 1] =
+ * l1_scale * sum |x - ref| over the owned elements of term t, in fp64.  Deterministic: per-block partial sums in a fixed order
+ * (work: n_terms * 2 * AERO_GAN_FWD_BLOCKS doubles), then one fixed-order reduction per term; no floating-point atomics.  A term
+ * whose geometry is invalid (n_seg, H or C < 1, halo < 0, halo + H > seg) yields NaN. */
+int aero_gan_loss_fwd(const aero_gan_term* terms, int32_t n_terms, double* out, double* work, aero_stream_t stream);
+
+/* Backward: writes every element of each term's dx -- owned elements get (float)adv_scale * adv'(x) + (float)l1_scale * sign(x - ref)
+ * (fp32; relu' and sign are 0 at their kinks, as in PyTorch), every other row exact 0.  Terms may share a dx buffer only on
+ * disjoint element ranges. */
+int aero_gan_loss_bwd(const aero_gan_term* terms, int32_t n_terms, aero_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
