@@ -31,7 +31,13 @@ struct TapGemmArgs {
 // tensor-core path: tile geometry and the fixed part of a CTA's shared memory, shared by the kernel and its launcher
 constexpr int kBM = 128;
 constexpr int kMaxStages = 8;
-constexpr int kMaxBN = 128;             // widest wgmma N used; wider layers take several n-tiles
+constexpr int kMaxBN = 128;             // widest tile of the narrow widths (32 .. 128): the whole accumulator tile is staged at once
+// Wide tiles (BN = 192 / 256, FP16 operands, long K loops; tapgemm_tc.cu pick_bn): one m64n192k16 / m64n256k16 per consumer
+// warpgroup and k-step.  The 96 / 128 accumulator registers per thread need setmaxnreg (producer warpgroup down to
+// kProducerRegs, consumers up to kConsumerRegs), and the accumulators go through the staging tile kSliceBN columns at a time.
+constexpr int kWideBN = 256;
+constexpr int kSliceBN = 64;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;      // 40 * 128 + 232 * 256 = 168 * 384: the launch's register file
 constexpr int kEpiWarps = 8;             // the two consumer warpgroups: two warps per 32-row quarter, alternating 16-column chunks
 constexpr int kThreads = 128 + 32 * kEpiWarps;
 constexpr int kATileBytes = kBM * 128;   // 16 KB

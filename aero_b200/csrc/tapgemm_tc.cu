@@ -15,6 +15,8 @@ KernelFn tapgemm_tc_kernels_bn32(bool f16a, bool f16o, int amode, bool res, bool
 KernelFn tapgemm_tc_kernels_bn64(bool f16a, bool f16o, int amode, bool res, bool stats);
 KernelFn tapgemm_tc_kernels_bn96(bool f16a, bool f16o, int amode, bool res, bool stats);
 KernelFn tapgemm_tc_kernels_bn128(bool f16a, bool f16o, int amode, bool res, bool stats);
+KernelFn tapgemm_tc_kernels_bn192(bool f16a, bool f16o, int amode, bool res, bool stats);
+KernelFn tapgemm_tc_kernels_bn256(bool f16a, bool f16o, int amode, bool res, bool stats);
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -88,22 +90,41 @@ int encode_map(CUtensorMap* out, const void* base, uint32_t rank, const uint64_t
     return AERO_OK;
 }
 
-// tile width: the narrowest built width (32, 64, 96, 128) that covers N in the fewest n-tiles
-static int pick_bn(int N) {
-    const int ntiles = (N + kMaxBN - 1) / kMaxBN;
-    const int per = (N + ntiles - 1) / ntiles;
-    return (per + 31) & ~31;
-}
-
 // Shared memory of a CTA besides the pipeline stages: barriers / scratch, the bias of every column (padded to whole tiles) and the
-// accumulator staging tile.
-static int tc_fixed_smem(int N, int BN) { return (int)sizeof(TcShared) + cdiv(N, BN) * BN * 4 + kBM * (BN + 4) * 4 + 1024; }
+// accumulator staging tile (the wide widths stage kSliceBN columns at a time).
+static int tc_fixed_smem(int N, int BN) {
+    return (int)sizeof(TcShared) + cdiv(N, BN) * BN * 4 + kBM * ((BN > kMaxBN ? kSliceBN : BN) + 4) * 4 + 1024;
+}
 // Pipeline depth: the producer runs ahead across tiles, so depth is set by bytes in flight, not by the K length: as many stages as
 // fit.  Fewer than two cannot run (a stage is released only after the next one's wgmmas are issued).
 static int tc_stages(int N, int BN) {
     if (N > (1 << 20)) return 0;
     const int st = (227 * 1024 - tc_fixed_smem(N, BN)) / (kATileBytes + BN * 128);
     return st > kMaxStages ? kMaxStages : st;
+}
+
+// Shortest K loop, (C1 + C2) x taps, that takes a wide tile.  A 128 x 256 tile halves the weight bytes each pixel tile pulls
+// and cuts the L2 -> SM bytes per FLOP by a quarter, which pays on the tensor-bound convolutions (the shortest of the
+// aero_4-16_512_64 forward is encoder.2.conv: 96 x 8 = 768).  The short-K launches (1x1 rewrites, LSTM gate inputs: K x taps
+// <= 384 there) are bound by HBM and by the epilogue; a wider tile only coarsens their waves, so they keep the narrow widths.
+constexpr int kWideMinKTaps = 512;
+
+// Tile width.  Narrow (32, 64, 96, 128): the narrowest that covers N in the fewest n-tiles of at most 128.  Wide (192, 256):
+// FP16 operands, N >= 192 and a K loop of at least kWideMinKTaps, when three pipeline stages and the statistics slots of a
+// tile still fit; otherwise the narrow width.
+static int pick_bn(const aero_tapgemm_params& p) {
+    const int nt = cdiv(p.N, kMaxBN);
+    const int narrow = (cdiv(p.N, nt) + 31) & ~31;
+    if (p.precision != 2 || p.mode == AERO_TAPS_MIX || p.N < 192) return narrow;
+    const int taps = (p.mode == AERO_TAPS_CONV) ? p.kf * p.kt : p.kf / p.stride_f;
+    if ((int64_t)(p.C1 + p.C2) * taps < kWideMinKTaps) return narrow;
+    const int bn = cdiv(p.N, cdiv(p.N, kWideBN)) <= 192 ? 192 : 256;
+    if (tc_stages(p.N, bn) < 3) return narrow;
+    if (p.stats_mode == 1) {
+        const int Nout = p.glu ? p.N / 2 : p.N;
+        if (p.groups < 1 || Nout % p.groups || (p.glu ? bn / 2 : bn) / (Nout / p.groups) + 2 > 8) return narrow;
+    }
+    return bn;
 }
 
 // precision 1: fp32 sources (tf32 wgmma); precision 2: FP16 sources (f16 wgmma).  TMA needs 16-byte global strides:
@@ -113,12 +134,12 @@ bool tapgemm_tc_eligible(const aero_tapgemm_params& p) {
     const int q = f16 ? 8 : 4;
     if (p.mode == AERO_TAPS_MIX)
         return p.w_sb == 0 && p.C1 % q == 0 && p.C2 == 0 && p.a1_st % q == 0 && p.a1_sb % q == 0 && p.N >= 8 &&
-               p.stats_mode == 0 && !p.glu && p.F_out == 1 && p.F_in == 1 && tc_stages(p.N, pick_bn(p.N)) >= 2;
+               p.stats_mode == 0 && !p.glu && p.F_out == 1 && p.F_in == 1 && tc_stages(p.N, pick_bn(p)) >= 2;
     if (p.w_sb != 0) return false;                                   // activations-as-weights (FTB frequency mix)
     if (p.act == AERO_ACT_TANH) return false;                        // tanh is built for the SIMT kernels only (SEANet's thin layers)
     if (p.act == AERO_ACT_LEAKY && (p.stats_mode != 0 || p.r_sb != 0 || p.r_sf != 0 || p.r_st != 0))
         return false;                                                // LeakyReLU: plain epilogue only (no residual, no statistics)
-    if (tc_stages(p.N, pick_bn(p.N)) < 2) return false;              // the bias of that many columns leaves no room for a pipeline
+    if (tc_stages(p.N, pick_bn(p)) < 2) return false;                // the bias of that many columns leaves no room for a pipeline
     if (p.N < 8) return false;                                       // thin outputs stay on the SIMT path
     const int K = p.C1 + p.C2;
     if (K < 8 || (p.C1 % q) || (p.C2 % q)) return false;
@@ -129,7 +150,7 @@ bool tapgemm_tc_eligible(const aero_tapgemm_params& p) {
         const int Nout = p.glu ? p.N / 2 : p.N;
         if (p.groups < 1 || Nout % p.groups) return false;
         const int gw = Nout / p.groups;
-        const int bn = pick_bn(p.N);
+        const int bn = pick_bn(p);
         if (gw % 8 || (p.glu ? bn / 2 : bn) / gw + 2 > 8) return false;
     }
     return true;
@@ -163,7 +184,7 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
     const bool f16a = p.precision == 2, f16o = (p.flags & AERO_TG_OUT_F16) != 0;
     const int esz = f16a ? 2 : 4, kBKc = 128 / esz;
     const int K = p.C1 + p.C2;
-    const int BN = pick_bn(p.N);
+    const int BN = pick_bn(p);
     const int nslab = (p.mode == AERO_TAPS_CONVT) ? p.kf : p.kf * p.kt;
     CUtensorMap mA1, mA2, mW;
     int rc;
@@ -220,7 +241,9 @@ int tapgemm_tc_launch(const TapGemmArgs& g0, cudaStream_t st) {
     const KernelFn kern = BN == 32 ? tapgemm_tc_kernels_bn32(f16a, f16o, amode, res, stats)
                         : BN == 64 ? tapgemm_tc_kernels_bn64(f16a, f16o, amode, res, stats)
                         : BN == 96 ? tapgemm_tc_kernels_bn96(f16a, f16o, amode, res, stats)
-                                   : tapgemm_tc_kernels_bn128(f16a, f16o, amode, res, stats);
+                        : BN == 128 ? tapgemm_tc_kernels_bn128(f16a, f16o, amode, res, stats)
+                        : BN == 192 ? tapgemm_tc_kernels_bn192(f16a, f16o, amode, res, stats)
+                                    : tapgemm_tc_kernels_bn256(f16a, f16o, amode, res, stats);
     if (!kern) {
         set_error("aero_tapgemm_fwd(wgmma): epilogue (act %d, residual %d, stats %d) is not built for operands %s / outputs %s",
                   amode, (int)res, (int)stats, f16a ? "f16" : "tf32", f16o ? "f16" : "f32");

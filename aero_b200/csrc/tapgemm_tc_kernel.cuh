@@ -7,8 +7,11 @@
 //   A tile : 128 pixels (consecutive t of one (b, f) row) x 128 bytes of channels = 128 rows, SWIZZLE_128B
 // One translation unit per tile width BN (tapgemm_tc_bn*.cu): the width is a template parameter because the accumulators of
 // every width a kernel could run would otherwise be allocated side by side and ptxas would serialise the wgmmas.
-//   B tile : BN <= 128 output columns x 128 bytes of channels (weights stored K-major [slab][N][K]) = BN rows
+//   B tile : BN <= 256 output columns x 128 bytes of channels (weights stored K-major [slab][N][K]) = BN rows
 //   D      : two warpgroups x (64 rows x BN fp32 columns) in registers
+// Narrow widths (BN <= 128) stage the whole accumulator tile in shared memory at once; the wide ones (192, 256: FP16 operands
+// only) stage and finish it kSliceBN columns at a time, so the staging tile stays at 128 x (kSliceBN + 4) floats and three
+// 48 KB pipeline stages still fit.
 // Persistent CTAs (one per SM) of three warpgroups: warp 0 of the first = TMA producer (runs ahead across tiles); the other
 // two each own 64 rows of the tile: they issue the wgmmas of the main loop, write their accumulators to a padded
 // shared-memory tile and then run the epilogue on it with two warps per 32-row quarter.  STAGES-deep mbarrier ring between
@@ -114,8 +117,8 @@ __device__ __forceinline__ void epilogue_stage_a(const uint32_t (&r)[16], uint32
 }
 
 template <int AMODE, bool RES, bool STATS, typename TO>
-__device__ __forceinline__ void epilogue_fast_tile(TcShared* sh, const TapGemmArgs& g, const TileCoord& tc, uint32_t tacc, int BN, int q,
-                                                   int ew, int lane, int Nout, int gw, int c_start, int c_step, uint32_t sbias) {
+__device__ __forceinline__ void epilogue_fast_tile(TcShared* sh, const TapGemmArgs& g, const TileCoord& tc, uint32_t tacc, int c_lo, int c_hi,
+                                                   int q, int ew, int lane, int Nout, int gw, int c_start, int c_step, uint32_t sbias) {
     const aero_tapgemm_params& p = g.p;
     constexpr int CNT = (AMODE == 3) ? 8 : 16;          // staged output columns per 16 accumulator columns
     constexpr int LPR = CNT / 4;                         // lanes per row (one float4 each)
@@ -131,12 +134,12 @@ __device__ __forceinline__ void epilogue_fast_tile(TcShared* sh, const TapGemmAr
     TO* const obase = static_cast<TO*>(g.out) + (int64_t)tc.b * p.o_sb + (int64_t)tc.fo * p.o_sf + (int64_t)row0 * p.o_st;
     const TO* const rbase = RES ? static_cast<const TO*>(g.residual) + (int64_t)tc.b * p.r_sb + (int64_t)tc.fo * p.r_sf + (int64_t)row0 * p.r_st : nullptr;
     const float* const adp = g.addend_fn ? g.addend_fn + (int64_t)tc.fo * Nout : nullptr;
-    for (int c0 = c_start; c0 < BN; c0 += c_step) {      // split mode: the two warps of a lane quarter alternate 16-column chunks
+    for (int c0 = c_lo + c_start; c0 < c_hi; c0 += c_step) {   // split mode: the two warps of a lane quarter alternate 16-column chunks
         const int nb = tc.n0 + c0;
         if (nb >= p.N) break;
         uint32_t r[16];
         if (tc.n_iters > 0) {
-            acc_ld16(tacc + 4u * (uint32_t)c0, r);
+            acc_ld16(tacc + 4u * (uint32_t)(c0 - c_lo), r);
         } else {
 #pragma unroll
             for (int j = 0; j < 16; ++j) r[j] = 0u;
@@ -208,8 +211,8 @@ __device__ __forceinline__ void epilogue_fast_tile(TcShared* sh, const TapGemmAr
 // and independent (bias / residual / addend loads issue together), which is what the HBM-bound layers need: with one or two
 // warps per scheduler the epilogue is a latency chain, not a throughput problem.
 template <int AMODE, bool RES, bool STATS, typename TO>
-__device__ __forceinline__ void epilogue_direct(TcShared* sh, const TapGemmArgs& g, const TileCoord& tc, uint32_t tacc, int BN, int q, int ew,
-                                                int lane, int Nout, int gw, int c_start, int c_step, uint32_t sbias) {
+__device__ __forceinline__ void epilogue_direct(TcShared* sh, const TapGemmArgs& g, const TileCoord& tc, uint32_t tacc, int c_lo, int c_hi, int q,
+                                                int ew, int lane, int Nout, int gw, int c_start, int c_step, uint32_t sbias) {
     const aero_tapgemm_params& p = g.p;
     constexpr int CNT = (AMODE == 3) ? 8 : 16;          // output columns per 16 accumulator columns
     constexpr bool F16 = sizeof(TO) == 2;
@@ -225,12 +228,12 @@ __device__ __forceinline__ void epilogue_direct(TcShared* sh, const TapGemmArgs&
     const int g_lo = ((AMODE == 3) ? tc.n0 >> 1 : tc.n0) / gw;
     int cur_g = -1;                                      // statistics: running group (warp-uniform), flushed when it changes
     float ssum = 0.f, ssq = 0.f;
-    for (int c0 = c_start; c0 < BN; c0 += c_step) {
+    for (int c0 = c_lo + c_start; c0 < c_hi; c0 += c_step) {
         const int nb = tc.n0 + c0;
         if (nb >= p.N) break;
         uint32_t r[16];
         if (tc.n_iters > 0) {
-            acc_ld16(tacc + 4u * (uint32_t)c0, r);
+            acc_ld16(tacc + 4u * (uint32_t)(c0 - c_lo), r);
         } else {
 #pragma unroll
             for (int j = 0; j < 16; ++j) r[j] = 0u;
@@ -327,13 +330,12 @@ __device__ __forceinline__ void epilogue_direct(TcShared* sh, const TapGemmArgs&
     }
 }
 
-// Main loop of one tile for one consumer warpgroup (rows 64 wg .. 64 wg + 63): n_iters pipeline stages of four wgmmas each, then
-// the accumulators go to rows of the staging tile (row stride `ldacc` floats).  A stage is handed back to the producer when
-// the wgmmas reading it have retired: one group stays in flight, so stage i - 1 is released after the wgmmas of stage i are issued.
+// Main loop of one tile for one consumer warpgroup (rows 64 wg .. 64 wg + 63): n_iters pipeline stages of four wgmmas each into
+// the accumulators d.  A stage is handed back to the producer when the wgmmas reading it have retired: one group stays in
+// flight, so stage i - 1 is released after the wgmmas of stage i are issued.
 template <int BN, bool F16A>
 __device__ __forceinline__ void tile_mainloop(TcShared* sh, uint8_t* smem, int& stage, uint32_t& phase, const int kStages, const int stage_bytes,
-                                              const int n_iters, const bool mix, const int wg, float* acc, const int ldacc) {
-    float d[BN / 2];            // first written by the first wgmma (scale-d = 0); never read when n_iters == 0
+                                              const int n_iters, const bool mix, const int wg, float (&d)[BN / 2]) {
     const int tid = threadIdx.x & 127, wl = tid >> 5, lane = tid & 31;
     int prev = -1;
     for (int i = 0; i < n_iters; ++i) {
@@ -383,11 +385,20 @@ __device__ __forceinline__ void tile_mainloop(TcShared* sh, uint8_t* smem, int& 
     }
     wgmma_wait<0>();
     if (prev >= 0 && tid == 0) mbar_arrive(&sh->empty[prev]);
+}
+
+// Accumulator columns [s0, s0 + SW) of this warpgroup -> its 64 rows of the staging tile (row stride SW + 4 floats).  s0 must
+// be known at compile time after unrolling: d lives in registers.
+template <int BN, int SW>
+__device__ __forceinline__ void stage_acc(const float (&d)[BN / 2], const int s0, float* acc, const int wg) {
+    constexpr int ldacc = SW + 4;
+    const int tid = threadIdx.x & 127, wl = tid >> 5, lane = tid & 31;
     float* row = acc + (wg * 64 + wl * 16 + (lane >> 2)) * ldacc + 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(row + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
-        *reinterpret_cast<float2*>(row + 8 * ldacc + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    for (int j = 0; j < SW / 8; ++j) {
+        const int jd = s0 / 8 + j;
+        *reinterpret_cast<float2*>(row + 8 * j) = make_float2(d[4 * jd], d[4 * jd + 1]);
+        *reinterpret_cast<float2*>(row + 8 * ldacc + 8 * j) = make_float2(d[4 * jd + 2], d[4 * jd + 3]);
     }
 }
 
@@ -404,15 +415,17 @@ tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_consta
     TcShared* sh = reinterpret_cast<TcShared*>(smem + kStages * stage_bytes);
     float* const sbias_f = reinterpret_cast<float*>(sh + 1);       // bias (or zeros), padded to whole 16-column chunks of the last tile
     const uint32_t sbias = smem_u32(sbias_f);
-    float* const acc = sbias_f + n_tiles * BN;                     // accumulator staging tile [128][BN + 4]
-    constexpr int ldacc = BN + 4;                                      // 16-byte rows; lane-per-row 16-byte reads hit distinct banks
+    constexpr bool kWide = BN > kMaxBN;
+    constexpr int kSW = kWide ? kSliceBN : BN;                     // columns staged at a time
+    float* const acc = sbias_f + n_tiles * BN;                     // accumulator staging tile [128][kSW + 4]
+    constexpr int ldacc = kSW + 4;                                     // 16-byte rows; lane-per-row 16-byte reads hit distinct banks
 
     using TO = typename std::conditional<F16O, __half, float>::type;
     constexpr int kBKc = OperandKind<F16A>::kBK;
     const aero_tapgemm_params& p = g.p;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nch1 = (p.C1 + kBKc - 1) / kBKc, nch2 = (p.C2 + kBKc - 1) / kBKc;
-    const bool mix = p.mode == AERO_TAPS_MIX;
+    const bool mix = !kWide && p.mode == AERO_TAPS_MIX;         // the host never gives a wide width to the row-mix mode
 
     for (int i = threadIdx.x; i < n_tiles * BN; i += kThreads) sbias_f[i] = (g.bias && i < g.p.N) ? g.bias[i] : 0.f;
     if (threadIdx.x == 0) {
@@ -423,9 +436,11 @@ tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_consta
     }
     __syncthreads();
 
-    if (warp == 0) {
-        // ===================================================== TMA producer
-        if (lane == 0) {
+    // wide tiles: the producer warpgroup hands registers to the consumers, whose accumulators take BN / 2 of them
+    if (warp < 4) {
+        if constexpr (kWide) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+        // ===================================================== TMA producer (warp 0)
+        if (warp == 0 && lane == 0) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA1) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
             int stage = 0;
@@ -469,7 +484,8 @@ tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_consta
                 }
             }
         }
-    } else if (warp >= 4) {
+    } else {
+        if constexpr (kWide) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
         // ===================================================== consumers (warpgroups 1, 2): main loop, then epilogue
         const int wg = (warp >> 2) - 1;                // 64-row half of the tile
         const int ew = warp - 4;                       // epilogue warp index
@@ -486,124 +502,131 @@ tapgemm_tc_kernel(const __grid_constant__ CUtensorMap mapA1, const __grid_consta
         for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x, ++local) {
             const TileCoord tc = tile_coord(g, tile, n_tiles, BN, nch1, nch2);
             const int b = tc.b, fo = tc.fo, t0 = tc.t0, n0 = tc.n0, n_iters = tc.n_iters;
-            tile_mainloop<BN, F16A>(sh, smem, stage, phase, kStages, stage_bytes, n_iters, mix, wg, acc, ldacc);
-            warpgroup_sync(1 + wg);                    // the staged rows of this half are complete
-            const uint32_t tacc = smem_u32(acc + m * ldacc);      // this lane's accumulator row
-            const int t = t0 + m;
-            const bool row_ok = t < p.T;
-            float sa = 1.f, sb = 0.f;
-            if (g.samp_affine) { sa = g.samp_affine[2 * b]; sb = g.samp_affine[2 * b + 1]; }
-            TO* op = static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + (int64_t)fo * p.o_sf + (int64_t)t * p.o_st;
-            const TO* rp = g.residual ? static_cast<const TO*>(g.residual) + (int64_t)b * p.r_sb + (int64_t)fo * p.r_sf + (int64_t)t * p.r_st : nullptr;
-            const float* csp = g.colscale ? g.colscale + (int64_t)b * p.cs_sb + (int64_t)t * p.cs_st : nullptr;
-            const float* adp = g.addend_fn ? g.addend_fn + (int64_t)fo * Nout : nullptr;
-            int cur_g = -1;
-            float ssum = 0.f, ssq = 0.f;
             const int g_lo = (p.glu ? n0 >> 1 : n0) / gw;
+            float d[BN / 2];            // first written by the first wgmma (scale-d = 0); never read when n_iters == 0
+            tile_mainloop<BN, F16A>(sh, smem, stage, phase, kStages, stage_bytes, n_iters, mix, wg, d);
+            // columns [s0, s0 + kSW) of the tile: staged, then finished by the epilogue (one pass for the narrow widths)
+#pragma unroll
+            for (int s0 = 0; s0 < BN; s0 += kSW) {
+                if (s0 > 0) warpgroup_sync(1 + wg);        // the previous slice is drained
+                stage_acc<BN, kSW>(d, s0, acc, wg);
+                warpgroup_sync(1 + wg);                    // the staged rows of this half are complete
+                const uint32_t tacc = smem_u32(acc + m * ldacc);      // this lane's accumulator row
+                const int t = t0 + m;
+                const bool row_ok = t < p.T;
+                float sa = 1.f, sb = 0.f;
+                if (g.samp_affine) { sa = g.samp_affine[2 * b]; sb = g.samp_affine[2 * b + 1]; }
+                TO* op = static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + (int64_t)fo * p.o_sf + (int64_t)t * p.o_st;
+                const TO* rp = g.residual ? static_cast<const TO*>(g.residual) + (int64_t)b * p.r_sb + (int64_t)fo * p.r_sf + (int64_t)t * p.r_st : nullptr;
+                const float* csp = g.colscale ? g.colscale + (int64_t)b * p.cs_sb + (int64_t)t * p.cs_st : nullptr;
+                const float* adp = g.addend_fn ? g.addend_fn + (int64_t)fo * Nout : nullptr;
+                int cur_g = -1;
+                float ssum = 0.f, ssq = 0.f;
 
-            if (mix) {
-                // transposed store: lane = pixel m (contiguous in memory), column = output row n
-                const float gate = (row_ok && g.colscale) ? g.colscale[(int64_t)b * p.cs_sb + t] : 1.f;
-                TO* ob = static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + t;
-                for (int c0 = c_start; c0 < BN; c0 += c_step) {
-                    uint32_t r[16];
-                    acc_ld16(tacc + 4u * (uint32_t)c0, r);
-                    if (row_ok) {
+                if (mix) {
+                    // transposed store: lane = pixel m (contiguous in memory), column = output row n
+                    const float gate = (row_ok && g.colscale) ? g.colscale[(int64_t)b * p.cs_sb + t] : 1.f;
+                    TO* ob = static_cast<TO*>(g.out) + (int64_t)b * p.o_sb + t;
+                    for (int c0 = c_start; c0 < BN; c0 += c_step) {
+                        uint32_t r[16];
+                        acc_ld16(tacc + 4u * (uint32_t)c0, r);
+                        if (row_ok) {
+#pragma unroll
+                            for (int j = 0; j < 16; ++j) {
+                                const int n = n0 + c0 + j;
+                                if (n < p.N) {
+                                    float x = __uint_as_float(r[j]) * gate;
+                                    if (rnd) x = round_tf32_rna(x);
+                                    stf(ob + (int64_t)n * p.o_st, x);
+                                }
+                            }
+                        }
+                    }
+                } else if (fast && (F16O ? (g.vec_o8 && (g.direct_f16 == 1 || (g.direct_f16 == 2 && AMODE == 3))) : g.direct_f32)) {
+                    epilogue_direct<AMODE, RES, STATS, TO>(sh, g, tc, tacc, s0, s0 + kSW, q, ew, lane, Nout, gw, c_start, c_step, sbias);
+                } else if (fast) {
+                    epilogue_fast_tile<AMODE, RES, STATS, TO>(sh, g, tc, tacc, s0, s0 + kSW, q, ew, lane, Nout, gw, c_start, c_step, sbias);
+                } else {
+                    // generic (unaligned outputs / colscale) epilogue: lane = row, scattered stores; one warp per 32-row quarter
+                    for (int c0 = s0; c0 < (grp == 0 ? s0 + kSW : s0); c0 += 16) {
+                        uint32_t r[16];
+                        if (n_iters > 0) {
+                            acc_ld16(tacc + 4u * (uint32_t)(c0 - s0), r);
+                        } else {
+#pragma unroll
+                            for (int j = 0; j < 16; ++j) r[j] = 0u;
+                        }
+                        const int nb = n0 + c0;
+                        if (nb >= p.N) continue;                   // uniform: padded columns of the last tile
+                        float v[16];
 #pragma unroll
                         for (int j = 0; j < 16; ++j) {
-                            const int n = n0 + c0 + j;
-                            if (n < p.N) {
-                                float x = __uint_as_float(r[j]) * gate;
-                                if (rnd) x = round_tf32_rna(x);
-                                stf(ob + (int64_t)n * p.o_st, x);
+                            const int n = nb + j;
+                            float x = __uint_as_float(r[j]);
+                            if (row_ok && n < p.N) {
+                                x += sbias_f[n];
+                                if (csp) x *= csp[n];
+                                if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
+                                else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
+                                else if (AMODE == 4) x = leaky_f(x);
                             }
+                            v[j] = x;
                         }
-                    }
-                }
-            } else if (fast && (F16O ? (g.vec_o8 && (g.direct_f16 == 1 || (g.direct_f16 == 2 && AMODE == 3))) : g.direct_f32)) {
-                epilogue_direct<AMODE, RES, STATS, TO>(sh, g, tc, tacc, BN, q, ew, lane, Nout, gw, c_start, c_step, sbias);
-            } else if (fast) {
-                epilogue_fast_tile<AMODE, RES, STATS, TO>(sh, g, tc, tacc, BN, q, ew, lane, Nout, gw, c_start, c_step, sbias);
-            } else {
-                // generic (unaligned outputs / colscale) epilogue: lane = row, scattered stores; one warp per 32-row quarter
-                for (int c0 = 0; c0 < (grp == 0 ? BN : 0); c0 += 16) {
-                    uint32_t r[16];
-                    if (n_iters > 0) {
-                        acc_ld16(tacc + 4u * (uint32_t)c0, r);
-                    } else {
+                        float o[16];
+                        int no0, cnt;
+                        if (p.glu) {
+                            no0 = nb >> 1;
+                            cnt = 8;
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) r[j] = 0u;
-                    }
-                    const int nb = n0 + c0;
-                    if (nb >= p.N) continue;                   // uniform: padded columns of the last tile
-                    float v[16];
+                            for (int j = 0; j < 8; ++j) o[j] = v[2 * j] * sigmoid_f(v[2 * j + 1]);
+                        } else {
+                            no0 = nb;
+                            cnt = 16;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int n = nb + j;
-                        float x = __uint_as_float(r[j]);
-                        if (row_ok && n < p.N) {
-                            x += sbias_f[n];
-                            if (csp) x *= csp[n];
-                            if (p.act == AERO_ACT_GELU) x = gelu_exact(x);
-                            else if (p.act == AERO_ACT_RELU) x = fmaxf(x, 0.f);
-                            else if (AMODE == 4) x = leaky_f(x);
+                            for (int j = 0; j < 16; ++j) o[j] = v[j];
                         }
-                        v[j] = x;
-                    }
-                    float o[16];
-                    int no0, cnt;
-                    if (p.glu) {
-                        no0 = nb >> 1;
-                        cnt = 8;
+                        // statistics bookkeeping is warp-uniform: groups depend on columns only
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] = v[2 * j] * sigmoid_f(v[2 * j + 1]);
-                    } else {
-                        no0 = nb;
-                        cnt = 16;
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) o[j] = v[j];
-                    }
-                    // statistics bookkeeping is warp-uniform: groups depend on columns only
-#pragma unroll
-                    for (int sub = 0; sub < 2; ++sub) {
-                        if (sub * 8 >= cnt) break;
-                        const int ns = no0 + sub * 8;
-                        if (p.stats_mode != 0 && ns < Nout) {
-                            const int gi = ns / gw;
-                            if (gi != cur_g) {
-                                if (cur_g >= 0) {
-                                    const float a = warp_sum(ssum), c = warp_sum(ssq);
-                                    if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] = a; sh->stats[ew][cur_g - g_lo][1] = c; }
+                        for (int sub = 0; sub < 2; ++sub) {
+                            if (sub * 8 >= cnt) break;
+                            const int ns = no0 + sub * 8;
+                            if (p.stats_mode != 0 && ns < Nout) {
+                                const int gi = ns / gw;
+                                if (gi != cur_g) {
+                                    if (cur_g >= 0) {
+                                        const float a = warp_sum(ssum), c = warp_sum(ssq);
+                                        if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] += a; sh->stats[ew][cur_g - g_lo][1] += c; }
+                                    }
+                                    cur_g = gi; ssum = 0.f; ssq = 0.f;
                                 }
-                                cur_g = gi; ssum = 0.f; ssq = 0.f;
+                            }
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) {
+                                const int jj = sub * 8 + j;
+                                const int nn = no0 + jj;
+                                if (row_ok && nn < Nout) {
+                                    float x = o[jj];
+                                    if (adp) x += adp[nn];
+                                    if (rp) x += ldf(rp + nn);
+                                    x = x * sa + sb;
+                                    if (rnd) x = round_tf32_rna(x);
+                                    x = stored(x, op);
+                                    o[jj] = x;
+                                    ssum += x;
+                                    ssq += x * x;
+                                }
                             }
                         }
+                        if (row_ok) {
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int jj = sub * 8 + j;
-                            const int nn = no0 + jj;
-                            if (row_ok && nn < Nout) {
-                                float x = o[jj];
-                                if (adp) x += adp[nn];
-                                if (rp) x += ldf(rp + nn);
-                                x = x * sa + sb;
-                                if (rnd) x = round_tf32_rna(x);
-                                x = stored(x, op);
-                                o[jj] = x;
-                                ssum += x;
-                                ssq += x * x;
-                            }
+                            for (int j = 0; j < 16; ++j)
+                                if (j < cnt && no0 + j < Nout) stf(op + no0 + j, o[j]);
                         }
                     }
-                    if (row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (j < cnt && no0 + j < Nout) stf(op + no0 + j, o[j]);
+                    if (p.stats_mode != 0 && cur_g >= 0) {
+                        const float a = warp_sum(ssum), c = warp_sum(ssq);
+                        if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] += a; sh->stats[ew][cur_g - g_lo][1] += c; }
                     }
-                }
-                if (p.stats_mode != 0 && cur_g >= 0) {
-                    const float a = warp_sum(ssum), c = warp_sum(ssq);
-                    if (lane == 0) { sh->stats[ew][cur_g - g_lo][0] = a; sh->stats[ew][cur_g - g_lo][1] = c; }
                 }
             }
             warpgroup_sync(1 + wg);                    // staging rows drained: the next tile may overwrite them
@@ -668,10 +691,14 @@ static KernelFn pick_kernel(int amode, bool res, bool stats) {
 }
 
 // The kernels of one tile width, chosen by operand kind, output type and epilogue; nullptr when that combination is not built.
+// The wide widths are built for FP16 operands only.
 template <int BN>
 static KernelFn pick_kernel_bn(bool f16a, bool f16o, int amode, bool res, bool stats) {
-    return f16a ? (f16o ? pick_kernel<BN, true, true>(amode, res, stats) : pick_kernel<BN, true, false>(amode, res, stats))
-                : (f16o ? pick_kernel<BN, false, true>(amode, res, stats) : pick_kernel<BN, false, false>(amode, res, stats));
+    if constexpr (BN > kMaxBN)
+        return !f16a ? nullptr : f16o ? pick_kernel<BN, true, true>(amode, res, stats) : pick_kernel<BN, true, false>(amode, res, stats);
+    else
+        return f16a ? (f16o ? pick_kernel<BN, true, true>(amode, res, stats) : pick_kernel<BN, true, false>(amode, res, stats))
+                    : (f16o ? pick_kernel<BN, false, true>(amode, res, stats) : pick_kernel<BN, false, false>(amode, res, stats));
 }
 
 }  // namespace aero
