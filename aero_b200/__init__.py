@@ -5,10 +5,12 @@ Public surface (mirrors the reference's ``src.models`` names):
   * ``Seanet``               -- drop-in for ``src.models.seanet.Seanet``
   * ``spectro`` / ``ispectro`` -- drop-ins for ``src.models.spec``
   * ``load_experiment``      -- Hydra-less reader of ``conf/experiment/*.yaml``
+  * ``resample``             -- ``torchaudio.functional.resample`` (default filter) on the GPU
 """
 from .model import Aero, AeroGeometry  # noqa: F401
 from .config import load_experiment, aero_kwargs, seanet_kwargs  # noqa: F401
 from .seanet import Seanet  # noqa: F401
+from .resampler import resample  # noqa: F401
 
 
 def spectro(x, n_fft=512, hop_length=None, pad=0, win_length=None):

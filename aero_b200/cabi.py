@@ -127,6 +127,7 @@ SYMBOLS = {
     "aero_local_attn_bwd": (C.c_int, [vp] * 5 + [C.POINTER(AttnParams), vp]),
     # SEANet generator
     "aero_seanet_input_fwd": (C.c_int, [vp, vp, vp, vp, C.POINTER(ResampleParams), vp]),
+    "aero_resample_fwd": (C.c_int, [vp, vp, vp, i64, i32, i32, i32, i32, i32, i32, vp]),
     "aero_reflect_act_fwd": (C.c_int, [vp, vp, i32, i32, i32, i64, i64, i32, i32, i32, vp]),
     "aero_reflect_act_bwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i64, i64, i32, i32, vp]),
     "aero_seanet_output_fwd": (C.c_int, [vp, vp, vp, vp, i32, i64, vp]),

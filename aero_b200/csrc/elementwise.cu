@@ -113,6 +113,9 @@ __global__ void __launch_bounds__(256) norm_act_kernel(const TI* x, const double
         } else if (OP == AERO_NA_GELU) {
 #pragma unroll
             for (int u = 0; u < 4; ++u) o[u] = gelu_exact(a[u]);
+        } else if (OP == AERO_NA_RELU) {
+#pragma unroll
+            for (int u = 0; u < 4; ++u) o[u] = fmaxf(a[u], 0.f);
         } else if (OP == AERO_NA_SNAKE) {
             const float al = snake_a[fin];
             const float ia = 1.0f / al;
@@ -216,6 +219,7 @@ extern "C" int aero_norm_act_fwd(const void* x, const double* stats, const float
         case AERO_NA_GELU: AERO_NA_LAUNCH(AERO_NA_GELU); break;
         case AERO_NA_GLU: AERO_NA_LAUNCH(AERO_NA_GLU); break;
         case AERO_NA_SNAKE: AERO_NA_LAUNCH(AERO_NA_SNAKE); break;
+        case AERO_NA_RELU: AERO_NA_LAUNCH(AERO_NA_RELU); break;
         case AERO_NA_GLU_SCALE_RES: AERO_NA_LAUNCH(AERO_NA_GLU_SCALE_RES); break;
         default: set_error("aero_norm_act_fwd: op=%d", p->op); return AERO_ERR_INVALID;
     }

@@ -1,4 +1,4 @@
-// SEANet input stage (reference src/models/seanet.py:158-168) and the reflection-halo pass that feeds its reflect-padded
+// SEANet input stage (reference src/models/seanet.py:158-168), torchaudio.functional.resample, and the reflection-halo pass that feeds its reflect-padded
 // convolutions (seanet.py:14-16,57-66,106-118).  See include/aero_b200.h for the contracts.
 #include "common.cuh"
 
@@ -47,6 +47,20 @@ __global__ void __launch_bounds__(kStatThreads) seanet_std_kernel(const float* _
     }
 }
 
+// Output sample t of one row of torchaudio.functional.resample's polyphase filter (_apply_sinc_resample_kernel): phase t % up
+// of filt[up][taps] over the input samples (t / up) * orig - width + k, zero outside [0, L_in), each divided by `den` first.
+__device__ __forceinline__ float polyphase_sample(const float* __restrict__ xs, const float* __restrict__ filt, int t, int L_in,
+                                                  int orig, int up, int width, int taps, float den) {
+    const int ph = t % up, s0 = (t / up) * orig - width;
+    const float* f = filt + (int64_t)ph * taps;
+    float v = 0.f;
+    for (int k = 0; k < taps; ++k) {
+        const int j = s0 + k;
+        if (j >= 0 && j < L_in) v = fmaf(f[k], xs[j] / den, v);
+    }
+    return v;
+}
+
 // one thread per written (clip, frame, channel): normalise, polyphase filter, zero pad, reflect into the halo
 __global__ void __launch_bounds__(256) seanet_resample_kernel(const float* __restrict__ x, const float* __restrict__ filt,
                                                               const float* __restrict__ affine, float* __restrict__ x0,
@@ -65,18 +79,20 @@ __global__ void __launch_bounds__(256) seanet_resample_kernel(const float* __res
         if (t < p.L_hr) {
             const float den = p.normalize ? p.floor_ + affine[2 * b] : 1.f;
             const float* xs = x + ((int64_t)b * p.C + c) * p.L_in;
-            if (p.up == 0) {
-                v = xs[t] / den;
-            } else {
-                const int ph = t % p.up, s0 = (t / p.up) * p.orig - p.width;
-                const float* f = filt + (int64_t)ph * p.taps;
-                for (int k = 0; k < p.taps; ++k) {
-                    const int j = s0 + k;
-                    if (j >= 0 && j < p.L_in) v = fmaf(f[k], xs[j] / den, v);
-                }
-            }
+            v = p.up == 0 ? xs[t] / den : polyphase_sample(xs, filt, t, p.L_in, p.orig, p.up, p.width, p.taps, den);
         }
         x0[((int64_t)b * rows + p.halo + u) * p.C + c] = v;
+    }
+}
+
+// torchaudio.functional.resample on rows of L_in samples: one thread per output sample
+__global__ void __launch_bounds__(256) resample_kernel(const float* __restrict__ x, const float* __restrict__ filt, float* __restrict__ y,
+                                                       int64_t rows, int L_in, int L_out, int orig, int up, int width, int taps) {
+    const int64_t n = rows * L_out;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / L_out;
+        const int t = (int)(i - r * L_out);
+        y[i] = polyphase_sample(x + r * L_in, filt, t, L_in, orig, up, width, taps, 1.f);
     }
 }
 
@@ -155,6 +171,20 @@ extern "C" int aero_seanet_input_fwd(const float* x, const float* filt, float* a
     if (rc != AERO_OK) return rc;
     seanet_resample_kernel<<<grid_for((int64_t)p.B * (p.L_valid + 2 * p.fill) * p.C), 256, 0, st>>>(x, filt, affine, x0, p);
     return check_launch("aero_seanet_input_fwd(resample)");
+}
+
+extern "C" int aero_resample_fwd(const float* x, const float* filt, float* y, int64_t rows, int32_t L_in, int32_t L_out, int32_t orig,
+                                 int32_t up, int32_t width, int32_t taps, aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(x && filt && y, "aero_resample_fwd: null argument");
+    AERO_REQUIRE(rows >= 1 && L_in >= 1 && L_out >= 1, "aero_resample_fwd: bad sizes (rows=%lld L_in=%d L_out=%d)", (long long)rows, L_in,
+                 L_out);
+    AERO_REQUIRE(orig >= 1 && up >= 1 && width >= 0 && taps >= 1, "aero_resample_fwd: bad filter (orig=%d up=%d width=%d taps=%d)", orig,
+                 up, width, taps);
+    AERO_REQUIRE((int64_t)L_out <= ((int64_t)L_in / orig + 1) * up, "aero_resample_fwd: L_out=%d exceeds the filter's %lld frames",
+                 L_out, (long long)(((int64_t)L_in / orig + 1) * up));
+    resample_kernel<<<grid_for(rows * L_out), 256, 0, (cudaStream_t)stream>>>(x, filt, y, rows, L_in, L_out, orig, up, width, taps);
+    return check_launch("aero_resample_fwd");
 }
 
 extern "C" int aero_reflect_act_fwd(const void* x, void* y, int32_t B, int32_t T, int32_t C, int64_t x_sb, int64_t y_sb,

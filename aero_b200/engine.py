@@ -16,11 +16,16 @@ import math
 import torch
 
 from . import cabi
-from .cabi import (ACT_GELU, ACT_NONE, ACT_RELU, NA_GELU, NA_GLU, NA_GLU_SCALE_RES, NA_SNAKE, TAPS_CONV,
+from .cabi import (ACT_GELU, ACT_NONE, ACT_RELU, NA_GELU, NA_GLU, NA_GLU_SCALE_RES, NA_RELU, NA_SNAKE, TAPS_CONV,
                    TAPS_CONVT)
 
 _LSTM_MAX_STEPS = 200      # reference modules.py:215 BLSTM(..., max_steps=200)
 _ATTN_HEADS, _ATTN_NDECAY = 4, 4   # reference modules.py:154 DConv(heads=4, ndecay=4)
+
+
+def dconv_norm_act_op(act_func):
+    """norm_act op of the DConv activation (reference modules.py:194-199): Snake, GELU, or ReLU for any other name."""
+    return {"snake": NA_SNAKE, "gelu": NA_GELU}.get(act_func, NA_RELU)
 
 
 def _ptr(t):
@@ -309,7 +314,8 @@ class AeroEngine:
                     o = f"{p}.dc{d}"
                     W[o + ".c1.w"], W[o + ".c1.b"] = pack_taps(sd[q + ".conv1.0.weight"]), sd[q + ".conv1.0.bias"].contiguous()
                     W[o + ".n1.g"], W[o + ".n1.b"] = sd[q + ".conv1.1.weight"].contiguous(), sd[q + ".conv1.1.bias"].contiguous()
-                    W[o + ".a"] = sd[q + ".act.a"].reshape(-1).contiguous()
+                    if kw["act_func"] == "snake":
+                        W[o + ".a"] = sd[q + ".act.a"].reshape(-1).contiguous()
                     W[o + ".c2.w"], W[o + ".c2.b"] = pack_taps(sd[q + ".conv2.0.weight"]), sd[q + ".conv2.0.bias"].contiguous()
                     W[o + ".n2.g"], W[o + ".n2.b"] = sd[q + ".conv2.1.weight"].contiguous(), sd[q + ".conv2.1.bias"].contiguous()
                     W[o + ".ls"] = sd[q + ".conv2.3.scale"].contiguous()
@@ -651,6 +657,7 @@ class AeroEngine:
         Fq, Cc = g.f_out, g.ch
         hid = int(Cc / kw["dconv_comp"])
         rows = B * Fq
+        act = dconv_norm_act_op(kw["act_func"])
         for d in range(abs(kw["dconv_depth"])):
             o = f"encoder.{g.index}.dc{d}"
             dil = 2 ** d if kw["dconv_depth"] > 0 else 1      # negative depth = no dilation (reference modules.py:176-177,201)
@@ -660,7 +667,7 @@ class AeroEngine:
             self._gemm(h_raw, W[o + ".c1.w"], a1=y, B=B, F_out=Fq, T=T, N=hid, C1=Cc, kt=3, dil_t=dil, pad_t=dil,
                        bias=W[o + ".c1.b"], stats=st1, stats_mode=2)
             self._norm_act(h_raw, st1, W[o + ".n1.g"], W[o + ".n1.b"], h, B=B, F_in=Fq, T=T, C_=hid, groups=1, scope=2,
-                           op=NA_SNAKE, snake_a=W[o + ".a"], rnd=True)
+                           op=act, snake_a=W.get(o + ".a"), rnd=True)
             if g.lstm:
                 self._blstm(h, W, o, rows, T, hid, f"{tag}.lstm")
             if g.attn:

@@ -1,7 +1,7 @@
 """Inference drivers with the reference's call shapes (SURVEY.md section 8a16, 8f rank 4).
 
 * ``get_estimate(model, lr_sig)``            -- reference ``src/enhance.py:11-15`` (no_grad forward).
-* ``enhance_long(model, lr_sig, sr, ...)``   -- what reference ``predict.py:56-86`` does to a whole file: cut it into
+* ``enhance_long(model, lr_sig, sr, ...)``   -- what reference ``predict.py:55-86`` does to a whole file: cut it into
   non-overlapping 10-second chunks, run the generator on each chunk on its own (each chunk is normalised by its own
   statistics, ``aero.py:462-464``) and concatenate.  The reference runs the chunks one by one at batch 1 with a
   host round trip per chunk; here equal-length chunks go through the kernels as one batch and stay on the device.
@@ -22,10 +22,16 @@ def get_estimate(model, lr_sig):
 
 
 @torch.no_grad()
-def enhance_long(model, lr_sig, sr, segment_sec=SEGMENT_DURATION_SEC, max_batch=8):
-    """lr_sig: [C, L] on the model's device, sampled at ``sr`` (= model.lr_sr).  Returns [C_out, ~L * scale]."""
+def enhance_long(model, lr_sig, sr, segment_sec=SEGMENT_DURATION_SEC, max_batch=8, upsample=False):
+    """lr_sig: [C, L] on the model's device, sampled at ``sr`` (= model.lr_sr).  Returns [C_out, ~L * scale].
+    ``upsample`` (the experiment's ``upsample: true``, reference predict.py:55-57): the whole signal is first resampled to
+    ``model.hr_sr`` on the device (``aero_b200.resample``) and then cut into chunks of ``hr_sr * segment_sec`` samples."""
     if lr_sig.dim() != 2:
         raise ValueError(f"expected [channels, samples], got {tuple(lr_sig.shape)}")
+    if upsample:
+        from .resampler import resample
+        lr_sig = resample(lr_sig, sr, model.hr_sr)
+        sr = model.hr_sr
     seg = int(sr * segment_sec)
     total = lr_sig.shape[-1]
     if total == 0 or seg <= 0:

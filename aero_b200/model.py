@@ -97,9 +97,16 @@ class _FreqTransform(_Holder):
                                    nn.BatchNorm2d(channels), nn.ReLU())
 
 
+def _dconv_act(act_func, nrows):
+    # reference src/models/modules.py:194-199,208: 'gelu' -> nn.GELU, 'snake' -> Snake(freq_dim), any other string -> nn.ReLU
+    if act_func == "snake":
+        return _SnakeParam(nrows)
+    return nn.GELU() if act_func == "gelu" else nn.ReLU()
+
+
 class _ResidualBranch(_Holder):
     # reference src/models/modules.py:152-219 (DConv); always GroupNorm(1, .)
-    def __init__(self, channels, compress, depth, init, lstm, attn, nrows, heads=4, ndecay=4):
+    def __init__(self, channels, compress, depth, init, lstm, attn, nrows, act_func, heads=4, ndecay=4):
         super().__init__()
         hidden = int(channels / compress)
         self.hidden, self.depth = hidden, abs(depth)
@@ -109,7 +116,7 @@ class _ResidualBranch(_Holder):
             blk = nn.ModuleDict()
             blk["conv1"] = nn.Sequential(nn.Conv1d(channels, hidden, 3, dilation=dil, padding=dil),
                                          nn.GroupNorm(1, hidden))
-            blk["act"] = _SnakeParam(nrows)
+            blk["act"] = _dconv_act(act_func, nrows)
             blk["conv2"] = nn.Sequential(nn.Conv1d(hidden, 2 * channels, 1), nn.GroupNorm(1, 2 * channels),
                                          nn.GLU(1), _Scale(channels, init))
             if lstm:
@@ -292,7 +299,8 @@ class Aero(nn.Module):
         self.end_iters, self.hybrid, self.hybrid_old, self.debug = end_iters, hybrid, hybrid_old, debug
         self.freq_emb = None
 
-        dconv_kw = dict(compress=dconv_comp, depth=dconv_depth, init=dconv_init)
+        self.act_func = act_func
+        dconv_kw = dict(compress=dconv_comp, depth=dconv_depth, init=dconv_init, act_func=act_func)
         self.encoder = nn.ModuleList()
         self.decoder = nn.ModuleList()
         for g in geom.layers:
@@ -313,7 +321,8 @@ class Aero(nn.Module):
     @staticmethod
     def _check_supported(kw):
         # The reference accepts more combinations than its shipped configs use; the CUDA
-        # path covers the spectral ("cac") frequency-only U-Net of conf/experiment/aero_*.yaml.
+        # path covers the spectral ("cac") frequency-only U-Net of conf/experiment/aero_*.yaml,
+        # with any DConv activation (act_func) and with or without spectral upsampling (spec_upsample).
         problems = []
         if not kw["cac"]:
             problems.append("cac=False")
@@ -321,12 +330,8 @@ class Aero(nn.Module):
             problems.append("rewrite=False")
         if kw["dconv_mode"] & 2:
             problems.append("dconv_mode with decoder DConv")
-        if kw["act_func"] != "snake":
-            problems.append(f"act_func={kw['act_func']!r}")
         if kw["context"] != 1 or kw["context_enc"] != 0:
             problems.append("context != 1 or context_enc != 0")
-        if not kw["spec_upsample"]:
-            problems.append("spec_upsample=False")
         if kw["nfft"] & (kw["nfft"] - 1) or not 64 <= kw["nfft"] <= 4096:
             problems.append("nfft must be a power of two in [64, 4096]")
         if problems:

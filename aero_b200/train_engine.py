@@ -23,7 +23,7 @@ import torch
 
 from . import cabi
 from .cabi import ACT_NONE, NA_GELU, NA_GLU, NA_GLU_SCALE_RES, NA_NO_NORM, NA_NONE, NA_RELU, NA_SNAKE, TAPS_CONV, TAPS_CONVT
-from .engine import _ATTN_HEADS, _ATTN_NDECAY, _LSTM_MAX_STEPS, pack_taps, tf32_round
+from .engine import _ATTN_HEADS, _ATTN_NDECAY, _LSTM_MAX_STEPS, dconv_norm_act_op, pack_taps, tf32_round
 
 _FTB_R, _FTB_RP = 5, 8          # FTB squeeze channels (modules.py:286) and their padded count (kernels work on channel quads)
 
@@ -611,14 +611,15 @@ class TrainEngine:
         Fq, Cc = g.f_out, g.ch
         hid = int(Cc / kw["dconv_comp"])
         rows = B * Fq
+        act = dconv_norm_act_op(kw["act_func"])
         for d in range(abs(kw["dconv_depth"])):
             q = f"encoder.{g.index}.dconv.layers.{d}"
             dil = 2 ** d if kw["dconv_depth"] > 0 else 1
             st1 = self._new(rows, 2, zero=True, dtype=torch.float64)
             h_raw = self.conv(y, None, Cc, 0, q + ".conv1.0.weight", q + ".conv1.0.bias", _Conv(kt=3, dil_t=dil, pad_t=dil), B, Fq, Fq, T, hid,
                               stats=st1, stats_mode=2)
-            h = self.norm_act(h_raw, NA_SNAKE, B=B, F_in=Fq, T=T, C_=hid, scope=2, gname=q + ".conv1.1.weight", bname=q + ".conv1.1.bias",
-                              stats=st1, snake=q + ".act.a")
+            h = self.norm_act(h_raw, act, B=B, F_in=Fq, T=T, C_=hid, scope=2, gname=q + ".conv1.1.weight", bname=q + ".conv1.1.bias",
+                              stats=st1, snake=q + ".act.a" if act == NA_SNAKE else None)
             if g.lstm:
                 h = self.blstm(h, q, rows, T, hid)
             if g.attn:

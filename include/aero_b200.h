@@ -181,12 +181,12 @@ int aero_sample_norm_fwd(const float* x, const double* stats, float* y, float* s
  * x : [B][F_in][T][C]; rows f_off .. f_off+F_out-1 are read (decoder crop, aero.py:209).
  * stats : fp64 {sum, sumsq}; scope 1: [B][groups] over F_in*T*(C/groups) values (uncropped);
  *         scope 2: [B*F_in][1] per row over T*C values (DConv's GroupNorm(1, C)).
- * op: AERO_NA_NONE y=g; AERO_NA_GELU; AERO_NA_GLU y[c]=g[c]*sigmoid(g[c+C/2]) (C_out=C/2);
+ * op: AERO_NA_NONE y=g; AERO_NA_GELU; AERO_NA_RELU y=max(g, 0); AERO_NA_GLU y[c]=g[c]*sigmoid(g[c+C/2]) (C_out=C/2);
  *     AERO_NA_SNAKE y = g + sin(a[f]*g)^2 / a[f];
  *     AERO_NA_GLU_SCALE_RES y[c] = residual[c] + scale[c] * glu(g)[c].
  */
 enum { AERO_NA_NONE = 0, AERO_NA_GELU = 1, AERO_NA_GLU = 2, AERO_NA_SNAKE = 3, AERO_NA_GLU_SCALE_RES = 4,
-       AERO_NA_RELU = 5, AERO_NA_LEAKY = 6 /* LeakyReLU(0.2) */, AERO_NA_TANH = 7 /* 5-7: training entry points only */ };
+       AERO_NA_RELU = 5, AERO_NA_LEAKY = 6 /* LeakyReLU(0.2) */, AERO_NA_TANH = 7 /* 6-7: training entry points only */ };
 enum { AERO_NA_NO_NORM = 16 };      /* aero_norm_act_params.flags, training entry points: skip the normalisation (activation only) */
 typedef struct {
     int32_t B, F_in, F_out, f_off, T, C;
@@ -437,6 +437,15 @@ typedef struct {
 } aero_resample_params;
 int aero_seanet_input_fwd(const float* x, const float* filt, float* affine, float* x0, const aero_resample_params* p,
                           aero_stream_t stream);
+
+/* Hann-windowed sinc resampling (the reference's data-pipeline resampler with its default filter) of `rows` independent
+ * signals: x [rows][L_in] -> y [rows][L_out], fp32,
+ *   y[r][t] = sum_k filt[t % up][k] * x[r][(t / up) * orig - width + k]   (k < taps; x is zero outside [0, L_in)),
+ * with filt[up][taps] the polyphase table of the reduced ratio orig:up (taps = 2*width + orig) and
+ * L_out <= (L_in / orig + 1) * up (the reference keeps ceil(up * L_in / orig)).  The same per-sample filter as
+ * aero_seanet_input_fwd. */
+int aero_resample_fwd(const float* x, const float* filt, float* y, int64_t rows, int32_t L_in, int32_t L_out, int32_t orig, int32_t up,
+                      int32_t width, int32_t taps, aero_stream_t stream);
 
 /* Reflection halo + activation (nn.ReflectionPad1d after nn.LeakyReLU, seanet.py:14-16,58-59):
  *   y(b, u, c) = act(x(b, r(u), c)),  u in [-halo, T + halo),  r(u) = |u| reflected at both ends (halo < T),
