@@ -97,6 +97,7 @@ SYMBOLS = {
     "aero_ftb_lin_squeeze_fwd": (C.c_int, [vp, vp, vp, vp, i32, C.POINTER(FtbLinParams), vp]),
     "aero_freq_mix_small_fwd": (C.c_int, [vp, vp, vp, vp, i32, i32, i64, i32, vp]),
     "aero_lstm_rec_fwd": (C.c_int, [vp, vp, vp, vp, C.POINTER(LstmParams), vp]),
+    "aero_lstm_tc_shape": (C.c_int, [i32, i32, i32, C.POINTER(i32)]),
     "aero_local_attn_fwd": (C.c_int, [vp, vp, C.POINTER(AttnParams), vp]),
     "aero_lsd_fwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "aero_stft_loss_fwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, vp]),

@@ -1,30 +1,26 @@
 // Persistent BiLSTM recurrence on the Hopper tensor cores (wgmma, sm_90a).  See include/aero_b200.h (aero_lstm_rec_fwd,
 // precision = 1).
 //
-// Per step the recurrent term is the small GEMM  D[gate rows x sequences] = W_hh[gate rows x H] * h^T[H x sequences]:
-//   A = W_hh, loaded ONCE by TMA into shared memory (K-major, SWIZZLE_128B) and resident for all steps.
-//       Gate rows are re-ordered into 128-row M tiles so that a thread finds the gates it needs in its
-//       own accumulator row (or one xor-16 shuffle away):
-//         GPT = 1 (64 < H <= 128): tile g holds gate g, lane = cell             -> 4 tiles, no exchange
-//         GPT = 2 (32 < H <=  64): tile t holds gates (2t, 2t+1); in every warp lanes 0-15 carry gate 2t
-//                                  and lanes 16-31 gate 2t+1 of the same 16 cells -> 2 tiles, one shfl.xor 16
-//   B = h of the previous step, written by the cell-update threads straight into the swizzled
-//       shared-memory operand layout, 16 sequences per CTA;
-//   operands are FP16 (K = 16 per wgmma): h is in (-1, 1) and W_hh is O(1), so FP16's 10-bit mantissa gives
-//       the same rounding as TF32 at half the shared-memory traffic and half the instruction count; accumulation is fp32;
-//   D = (4/GPT) tiles of 128 rows x 16 fp32 columns: the MMA warpgroup holds them in registers (two m64n16 accumulators per
-//       tile), writes them to a padded shared-memory tile and the cell-update threads read their row back.
-// The input-projection gate pre-activations keep PyTorch's [dir][i,f,g,o][H] column order (a warp reads the contiguous
-// cells of one gate per sequence); with one CTA per SM (GPT = 1) they are requested a whole step ahead.
-// A CTA owns SEQ = 8 or 16 sequences (the wgmma N stays 16; unused operand rows are zero).  With 8, W_hh for 64 < H <= 96 is
-// held in 32-column SWIZZLE_64B chunks (96 KB instead of 128 KB, no zero K padding: 3/4 of the wgmmas per step) and the
-// sequences spread over twice as many SMs; for H <= 64 two CTAs share an SM and one CTA's MMA / barrier latency overlaps
-// the other's exp-heavy cell update.
-// Warps 0..3 are the MMA warpgroup (warp 0 also loads W_hh) and issue the wgmmas from step-invariant descriptors; two mbarriers ping-pong between
-// "h ready" and "accumulators ready".  c stays in registers for the whole sequence.  8 (GPT = 2) or 16 (GPT = 1)
-// cell-update warps; in the two-gates-per-tile layout a lane finishes only its own half of the warp's sequences.
+// Per step the recurrent term is the small GEMM  D[4H gate rows x sequences] = W_hh[4H x H] * h^T[H x sequences]:
+//   A = W_hh, FP16, held in REGISTERS as the wgmma A fragment for the whole sequence.  The 4H gate rows are packed densely in
+//       PyTorch's order, dense row R = gate * H + cell, into KS = ceil(4H / 64) = ceil(H / 16) m64 tiles; K = H runs in KS
+//       k16 steps (zero beyond H).  Tile t, k-step k is 4 registers per thread; one MMA warpgroup holds all tiles when
+//       KS <= 4 (H <= 64: 4 x 4 x 4 = 64 registers, 36 at H = 48), two warpgroups split them when KS <= 6 (H <= 96: 3 x 6 x 4 = 72
+//       each).  They are gathered once per CTA from the re-ordered rows lstm_gate_reorder / lstm_whh_fp16 produce (L2-resident,
+//       4-byte loads), so no shared-memory traffic for A remains in the step;
+//   B = h of the previous step, FP16, written by the cell-update threads straight into the swizzled (SWIZZLE_128B, K-major)
+//       shared-memory operand layout, one NT x 64-column tile per 64 cells (NT = wgmma N = 8 or 16 sequences);
+//   D = KS tiles of 64 x NT fp32 (accumulated in fp32; only the order of the K sum differs from a plain dot product), staged
+//       transposed in shared memory, sAcc[sequence][R] with a row stride of 64 KS + 4 floats: the MMA threads' scalar stores and
+//       the cell threads' float2 reads of two adjacent cells of one gate are both free of bank conflicts.
+// Two sequence groups per CTA (ping-pong): the MMA warpgroup(s) serve group 0 and group 1 alternately, so one group's wgmmas run
+// while the other group's cell warps do their exp-heavy update.  Each group has its own h_ready / acc_ready mbarrier pair, B
+// operand and staging buffer, and four cell-update warps.  A cell thread owns up to kItems (sequence, cell pair) items of its
+// group, two adjacent cells each, and only live cells (< H) are computed: gate pre-activations load as float2 / half2 (the
+// input projection keeps PyTorch's [dir][i,f,g,o][H] column order) and are requested into registers a whole step ahead and into
+// L2 two steps ahead; c stays in registers.
 #include <cuda_fp16.h>
-#include <cstdlib>
+#include <algorithm>
 #include "tc_common.cuh"
 
 #ifdef AERO_TC_TRACE
@@ -39,19 +35,16 @@ extern "C" int aero_debug_lstm_trace(long long* host) {
 
 namespace aero {
 
-constexpr int kNT = 16;          // wgmma N (operand rows of h); a CTA fills SEQ = 8 or 16 of them
-constexpr int kLdAcc = kNT + 4;  // row stride (floats) of the staged accumulators: lane-per-row 16-byte reads hit distinct banks
+constexpr int kCellThreads = 128;   // cell-update threads per sequence group
+constexpr int kItems = 3;           // cell pairs per cell thread (all of one sequence)
 
-// tuning knob, read from the environment once: AERO_LSTM_SEQ = 8 / 16 forces the CTA size (0 / unset: chosen per launch)
-static int lstm_seq_knob() {
-    static const int v = [] { const char* e = getenv("AERO_LSTM_SEQ"); return e ? atoi(e) : 0; }();
-    return v;
-}
+struct LstmTcShape {
+    int S, nt, ctas_per_dir, tps;       // sequences per group, wgmma N, CTAs per direction, cell threads per sequence
+};
 
 struct LstmTcShared {
-    uint64_t w_full;
-    uint64_t acc_ready;
-    uint64_t h_ready;
+    uint64_t acc_ready[2];
+    uint64_t h_ready[2];
 };
 
 // ex2.approx / rcp.approx: <= 2 ulp each, i.e. ~1e-7 relative on the gates (far below the operand rounding)
@@ -66,301 +59,284 @@ __device__ __forceinline__ float fast_rcp(float x) {
     return y;
 }
 
-template <typename T> __device__ __forceinline__ T to_storage(float v);
-template <> __device__ __forceinline__ float to_storage<float>(float v) { return v; }
-template <> __device__ __forceinline__ __half to_storage<__half>(float v) { return __float2half_rn(v); }
+__device__ __forceinline__ float2 ld2f(const float* p) { return *reinterpret_cast<const float2*>(p); }
+__device__ __forceinline__ float2 to_f2(float2 v) { return v; }
+__device__ __forceinline__ float2 to_f2(__half2 v) { return __half22float2(v); }
+template <typename TG> struct Pair;
+template <> struct Pair<float> { using T = float2; };
+template <> struct Pair<__half> { using T = __half2; };
+__device__ __forceinline__ void st2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
+__device__ __forceinline__ void st2(__half* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = pack_half2_sat(a, b); }
 
-// GPT: gates per 128-row tile.  NEW: cell-update warps (NEW/4 per 32-row quarter of a tile, each owning 4*SEQ/NEW sequences).
-// SEQ: sequences per CTA (8 or 16).  ROWB: bytes of K per operand row of a chunk (128 = 64 fp16, SWIZZLE_128B; 64 = 32 fp16,
-// SWIZZLE_64B).  MINB: CTAs per SM the register budget is set for.
-template <int GPT, int NEW, int SEQ, int ROWB, int MINB, typename TO, typename TG>
-__global__ void __launch_bounds__(128 + 32 * NEW, MINB)
-lstm_tc_kernel(const __grid_constant__ CUtensorMap mapW, const TG* __restrict__ gin, const float* __restrict__ bias_pad,
-               TO* __restrict__ hout, const aero_lstm_params p, const int nK) {
-    constexpr int NM = 4 / GPT;                          // M tiles
-    constexpr int CPW = 32 / GPT;                        // cells per warp
-    constexpr int kNS = 4 * SEQ / NEW;                   // sequences per cell-update warp
-    constexpr int kATile = 128 * ROWB, kBTile = kNT * ROWB, kKC = ROWB / 2;   // bytes per A / B chunk tile, fp16 of K per chunk
+// KS = ceil(H / 16): m64 tiles of gate rows == k16 steps of K.  NT: wgmma N (8 or 16 sequences per group).
+template <int KS> struct LstmTcCfg {
+    static constexpr int kWG = KS > 4 ? 2 : 1;                  // MMA warpgroups
+    static constexpr int kTW = (KS + kWG - 1) / kWG;            // m64 tiles per MMA warpgroup (KS = 5: the last one is zero)
+    static constexpr int kLdr = 64 * kWG * kTW + 4;             // staged accumulator row stride (floats), == 4 mod 32
+    static constexpr int kThreads = 128 * kWG + 2 * kCellThreads;
+};
+
+template <int KS, int NT, typename TO, typename TG>
+__global__ void __launch_bounds__(LstmTcCfg<KS>::kThreads, 1)
+lstm_tc_kernel(const __half* __restrict__ whh, const TG* __restrict__ gin, const float* __restrict__ bias_pad,
+               TO* __restrict__ hout, const aero_lstm_params p, const int S, const int tps) {
+    using Cfg = LstmTcCfg<KS>;
+    constexpr int kTW = Cfg::kTW, kLdr = Cfg::kLdr, NWG = Cfg::kWG;
+    constexpr int nK = (KS + 3) / 4;                    // 64-column B chunks
+    constexpr int kBTile = NT * 128;                    // bytes of one 64-column B chunk (NT rows of 128 B)
+    using TG2 = typename Pair<TG>::T;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* sA = smem;                                  // [NM][nK] tiles of 128 rows x ROWB bytes
-    uint8_t* sB = smem + NM * nK * kATile;               // [nK] tiles of 16 rows x ROWB bytes
-    float* sAcc = reinterpret_cast<float*>(sB + nK * kBTile);   // [NM][128][kLdAcc] staged accumulators
-    LstmTcShared* sh = reinterpret_cast<LstmTcShared*>(sAcc + NM * 128 * kLdAcc);
+    const int H = p.H;
+    uint8_t* sB = smem;                                 // [2][nK][kBTile]
+    float* sAcc = reinterpret_cast<float*>(sB + 2 * nK * kBTile);   // [2][NT][kLdr]
+    LstmTcShared* sh = reinterpret_cast<LstmTcShared*>(sAcc + 2 * NT * kLdr);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.y;
-    const int seq0 = blockIdx.x * SEQ;
     const int n_seq = p.rows * p.n_win;
-    const int H = p.H;
-    const int ldg = 8 * H;                               // floats per gin row: [dir][i,f,g,o][H], PyTorch's own order
+    // group g of this CTA: sequences [seq0 + g * S, + live[g]); group 0 is never empty, group 1 may be
+    const int seq0 = blockIdx.x * 2 * S;
+    const int live0 = min(S, n_seq - seq0), live1 = max(0, min(S, n_seq - seq0 - S));
 
     if (threadIdx.x == 0) {
-        mbar_init(&sh->w_full, 1);
-        mbar_init(&sh->acc_ready, 128);
-        mbar_init(&sh->h_ready, 32 * NEW);
+        for (int g = 0; g < 2; ++g) {
+            mbar_init(&sh->acc_ready[g], 128 * NWG);
+            mbar_init(&sh->h_ready[g], max(1, (g ? live1 : live0) * tps));   // the cell threads that own a sequence
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int i = threadIdx.x; i < nK * kBTile / 4; i += blockDim.x) reinterpret_cast<float*>(sB)[i] = 0.f;
+    for (int i = threadIdx.x; i < 2 * nK * kBTile / 4; i += blockDim.x) reinterpret_cast<float*>(sB)[i] = 0.f;
     fence_proxy_async_smem();
     __syncthreads();
 
-    if (warp < 4) {
-        if (threadIdx.x == 0) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW) : "memory");
-            mbar_expect_tx(&sh->w_full, (uint32_t)(NM * nK * kATile));
-            for (int m = 0; m < NM; ++m)
-                for (int kc = 0; kc < nK; ++kc)
-                    tma_load_2d(sA + (m * nK + kc) * kATile, &mapW, &sh->w_full, kc * kKC, (dir * NM + m) * 128);
-        }
-        // MMA warpgroup.  Every descriptor is step-invariant, so they are built once; only the low bits change along K
-        // (+2 per 32 bytes) and with the 64-row half of a tile.
-        constexpr int kMaxKC = (ROWB == 128) ? 2 : 4;     // H <= 128
-        uint64_t da[NM][kMaxKC], db[kMaxKC];
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
+    if (warp < 4 * NWG) {
+        // ===================================================== MMA warpgroup(s)
+        const int wg = warp >> 2, wl = warp & 3;
+        // A fragment of m64k16 (FP16): reg r of lane l holds rows 16 wl + l/4 (+8 if r odd), columns 2 (l%4) (+8 if r >= 2), +1.
+        // Dense row R = gate * H + cell comes from the re-ordered row of lstm_gate_reorder (GPT = 1 if H > 64 else 2).
+        const int kp = 64 * nK;                         // fp16 per re-ordered row
+        const int nM = H > 64 ? 4 : 2;
+        uint32_t a[kTW][KS][4];
 #pragma unroll
-        for (int kc = 0; kc < kMaxKC; ++kc) {
-            db[kc] = make_desc_kmajor<ROWB>(b0 + (uint32_t)(kc * kBTile));
+        for (int lt = 0; lt < kTW; ++lt)
 #pragma unroll
-            for (int m = 0; m < NM; ++m) da[m][kc] = make_desc_kmajor<ROWB>(a0 + (uint32_t)((m * nK + kc) * kATile));
-        }
-        float* const arow = sAcc + (warp * 16 + (lane >> 2)) * kLdAcc + 2 * (lane & 3);
-        mbar_wait(&sh->w_full, 0);
-        for (int s = 1; s < p.steps; ++s) {
-            mbar_wait(&sh->h_ready, (uint32_t)((s - 1) & 1));
-            LSTM_TRACE(0, s);
-            float d[NM][2][8];          // first written by the first wgmma of each chain (scale-d = 0)
-            wgmma_fence();
+            for (int k = 0; k < KS; ++k)
 #pragma unroll
-            for (int m = 0; m < NM; ++m) {
-#pragma unroll
-                for (int hf = 0; hf < 2; ++hf) {
-#pragma unroll
-                    for (int kc = 0; kc < kMaxKC; ++kc) {
-                        if (kc < nK) {
-#pragma unroll
-                            for (int k = 0; k < ROWB / 32; ++k)        // K = 16 fp16 = 32 B per wgmma
-                                Wgmma<kNT, true, 0>::ss(d[m][hf], da[m][kc] + (uint64_t)(hf * ((64 * ROWB) >> 4) + 2 * k), db[kc] + 2 * k,
-                                                        (kc == 0 && k == 0) ? 0u : 1u);
-                        }
+                for (int r = 0; r < 4; ++r) {
+                    const int R = (wg * kTW + lt) * 64 + wl * 16 + (lane >> 2) + 8 * (r & 1);
+                    const int col = 16 * k + 2 * (lane & 3) + 8 * (r >> 1);
+                    uint32_t v = 0u;
+                    if (R < 4 * H && col < H) {
+                        const int gate = R / H, cell = R - gate * H;
+                        const int src = H > 64 ? gate * 128 + cell
+                                               : (gate >> 1) * 128 + (cell >> 4) * 32 + (gate & 1) * 16 + (cell & 15);
+                        v = __ldg(reinterpret_cast<const uint32_t*>(whh + (size_t)(dir * nM * 128 + src) * kp + col));
                     }
+                    a[lt][k][r] = v;
                 }
+        // B descriptors: group g, k-step k -> chunk k / 4, +32 bytes per k16 inside the 128-byte swizzled row
+        const uint64_t db0 = make_desc_kmajor<128>(smem_u32(sB));
+        const int ng = live1 > 0 ? 2 : 1;
+        float* const arow = sAcc + 2 * (lane & 3) * kLdr + wg * kTW * 64 + wl * 16 + (lane >> 2);
+        for (int s = 1; s < p.steps; ++s) {
+            for (int g = 0; g < ng; ++g) {
+                mbar_wait(&sh->h_ready[g], (uint32_t)((s - 1) & 1));
+                if (g == 0) LSTM_TRACE(0, s);
+                const uint64_t db = db0 + (uint64_t)(g * ((nK * kBTile) >> 4));
+                float d[kTW][NT / 2];      // first written by the first wgmma of each chain (scale-d = 0)
+                wgmma_fence();
+#pragma unroll
+                for (int lt = 0; lt < kTW; ++lt)
+#pragma unroll
+                    for (int k = 0; k < KS; ++k)
+                        Wgmma<NT, true, 0>::rs(d[lt], a[lt][k], db + (uint64_t)((k >> 2) * (kBTile >> 4) + 2 * (k & 3)), k == 0 ? 0u : 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                float* const acc = arow + g * NT * kLdr;
+#pragma unroll
+                for (int lt = 0; lt < kTW; ++lt)
+#pragma unroll
+                    for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                            acc[(8 * j + (e & 1)) * kLdr + lt * 64 + 8 * (e >> 1)] = d[lt][4 * j + e];
+                mbar_arrive(&sh->acc_ready[g]);
+                if (g == 0) LSTM_TRACE(1, s);
             }
-            wgmma_commit();
-            wgmma_wait<0>();
-#pragma unroll
-            for (int m = 0; m < NM; ++m)
-#pragma unroll
-                for (int hf = 0; hf < 2; ++hf)
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) {
-                        float* r = arow + (m * 128 + hf * 64) * kLdAcc + 8 * j;
-                        *reinterpret_cast<float2*>(r) = make_float2(d[m][hf][4 * j], d[m][hf][4 * j + 1]);
-                        *reinterpret_cast<float2*>(r + 8 * kLdAcc) = make_float2(d[m][hf][4 * j + 2], d[m][hf][4 * j + 3]);
-                    }
-            mbar_arrive(&sh->acc_ready);
-            LSTM_TRACE(1, s);
         }
     } else {
-        // ===================================================== cell update (warps 4..4+NEW)
-        const int ew = warp - 4;
-        const int q = warp & 3;                          // 32-row quarter of every tile
-        const int wp = ew >> 2;                          // which slice of the 16 sequences
-        const int sub = lane / CPW;                      // gate slot inside the tile (0 for GPT=1)
-        const int cell = q * CPW + (lane % CPW);
-        const bool cell_ok = cell < H;
-        const int r = q * 32 + lane;                     // accumulator row == gin column inside a tile
+        // ===================================================== cell update: four warps per group
+        const int g = (warp - 4 * NWG) >> 2;
+        const int t = threadIdx.x - 128 * NWG - g * kCellThreads;
+        // thread t: local sequence n = t / tps, cell pairs pp + tps j (j < kItems, pair < H / 2): cells 2 pair, 2 pair + 1
+        const int n = t / tps, pp = t - n * tps;
+        if (n >= (g ? live1 : live0)) return;
+        const int hp = H >> 1;
         const int half = p.win_stride / 2;
         const int dpos = dir ? -1 : 1;
         const int pos0 = dir ? p.steps - 1 : 0;
+        const int ldg = 8 * H;                          // gin row: [dir][i,f,g,o][H], PyTorch's own order
 
-        // Per-sequence state, all loop-invariant work hoisted (32-bit element offsets; the host checks they fit).
         // A step s reads the input projection iff (unsigned)(s - g_lo) < g_len (else the frame is zero padding: bias only)
         // and writes its output iff (unsigned)(s - w_lo) < w_len (window crop of modules.py:53-59 and the T limit).
-        // For GPT=2 lane<16 updates even local sequences, lane>=16 odd ones.
-        // A lane reads gate pre-activations for all kNS sequences of its warp, but finishes (cell state, h, stores) only
-        // kMS = kNS / GPT of them: sequence i = ii*GPT + sub (GPT == 2: the partner lane xor 16 finishes the others).
-        // gate pre-activation column of this lane in tile 0 (tile m adds m * GPT * H): gate = m*GPT + sub, this lane's cell
-        // (clamped for the padding lanes of the last cells: their values are never used)
-        const int gcol = dir * 4 * H + sub * H + min(cell, H - 1);
-        const int gtile = GPT * H;
-        constexpr int kMS = kNS / GPT;
-        int goff[kNS], g_lo[kNS], g_len[kNS];
-        int ooff[kMS], w_lo[kMS], w_len[kMS];
-        uint32_t baddr[kMS];
-        const int jq = (cell & (kKC - 1)) >> 3;                              // 16-byte unit of this cell inside its chunk row
-        const uint32_t bbase = smem_u32(sB) + (uint32_t)((cell / kKC) * kBTile + ((cell & 7) << 1));
-#pragma unroll
-        for (int i = 0; i < kNS; ++i) {
-            const int n = wp * kNS + i;
-            const int sq = min(seq0 + n, n_seq - 1);
-            const int row = sq / p.n_win, k = sq - row * p.n_win;
-            const int f0 = k * p.win_stride;                               // first frame of the window
-            goff[i] = (p.in_windowed ? (sq * p.steps + pos0) : (row * p.T + f0 + pos0)) * ldg + gcol;
-            // valid input positions of this window: frames < T.  position -> step: dir 0: s = pos; dir 1: s = steps-1-pos
-            const int in_hi = p.in_windowed ? p.steps : max(0, min(p.steps, p.T - f0));
-            g_lo[i] = dir ? p.steps - in_hi : 0;
-            g_len[i] = in_hi;
+        const int sq = seq0 + g * S + n;
+        const int row = sq / p.n_win, k = sq - row * p.n_win;
+        const int f0 = k * p.win_stride;                                  // first frame of the window
+        const int cell0 = 2 * pp, cstep = 2 * tps;                        // cells of item j: cell0 + cstep j, +1
+        const int gcol = dir * 4 * H + cell0;
+        int goff = (p.in_windowed ? (sq * p.steps + pos0) : (row * p.T + f0 + pos0)) * ldg + gcol;
+        // valid input positions of this window: frames < T.  position -> step: dir 0: s = pos; dir 1: s = steps-1-pos
+        const int in_hi = p.in_windowed ? p.steps : max(0, min(p.steps, p.T - f0));
+        const int g_lo = dir ? p.steps - in_hi : 0, g_len = in_hi;
+        int ooff = (p.out_windowed ? (sq * p.steps + pos0) : (row * p.T + f0 + pos0)) * 2 * H + dir * H + cell0;
+        // kept output positions [lo, hi) (window crop of modules.py:53-59) intersected with frames < T
+        int lo = 0, hi = p.steps;
+        if (!p.out_windowed) {
+            lo = (k == 0) ? 0 : half;
+            hi = min((k == p.n_win - 1) ? p.steps : p.steps - half, p.T - f0);
         }
+        const int w_lo = dir ? p.steps - hi : lo, w_len = max(0, hi - lo);
+        const float* const accn = sAcc + (g * NT + n) * kLdr + cell0;
+        bool ok[kItems];
+        uint32_t baddr[kItems];
 #pragma unroll
-        for (int ii = 0; ii < kMS; ++ii) {
-            const int n = wp * kNS + ii * GPT + sub;
-            const int sq = min(seq0 + n, n_seq - 1);
-            const bool exists = seq0 + n < n_seq;
-            const int row = sq / p.n_win, k = sq - row * p.n_win;
-            const int f0 = k * p.win_stride;
-            ooff[ii] = (p.out_windowed ? (sq * p.steps + pos0) : (row * p.T + f0 + pos0)) * 2 * H + dir * H + cell;
-            // kept output positions [lo, hi) (window crop of modules.py:53-59) intersected with frames < T
-            int lo = 0, hi = p.steps;
-            if (!p.out_windowed) {
-                lo = (k == 0) ? 0 : half;
-                hi = min((k == p.n_win - 1) ? p.steps : p.steps - half, p.T - f0);
-            }
-            if (!exists || !cell_ok) hi = lo;
-            w_lo[ii] = dir ? p.steps - hi : lo;
-            w_len[ii] = max(0, hi - lo);
-            // swizzled B-operand address of (sequence n, k = cell), fp16: chunk tile cell / kKC, row n (ROWB bytes), 16-byte unit
-            // jq XOR-ed with the row (SWIZZLE_128B: n % 8; SWIZZLE_64B: (n / 2) % 4)
-            baddr[ii] = bbase + (uint32_t)((n >> 3) * (8 * ROWB) + (n & 7) * ROWB + ((jq ^ (ROWB == 128 ? (n & 7) : ((n >> 1) & 3))) << 4));
+        for (int j = 0; j < kItems; ++j) {
+            ok[j] = pp + tps * j < hp;
+            // swizzled B-operand address of (sequence n, k = cell), fp16: chunk cell / 64, row n (128 B), 16-byte unit
+            // (cell % 64) / 8 XOR-ed with n % 8, then (cell % 8) * 2 bytes
+            const int cell = cell0 + cstep * j;
+            baddr[j] = smem_u32(sB) + (uint32_t)((g * nK + (cell >> 6)) * kBTile + (n >> 3) * 1024 + (n & 7) * 128 +
+                                                 ((((cell & 63) >> 3) ^ (n & 7)) << 4) + ((cell & 7) << 1));
         }
-        const float* bptr = bias_pad + gcol;
         const int gstep = dpos * ldg, ostep = dpos * 2 * H;
 
-        float c_state[kMS];
+        float c_state[kItems][2];
+        TG2 gn[kItems][4];      // next step's gate pre-activations, kept in the storage type until the step that uses them
 #pragma unroll
-        for (int i = 0; i < kMS; ++i) c_state[i] = 0.f;
-
-        // The input-projection gate pre-activations stream from HBM (hundreds of MB per layer); their ~1 us load latency must
-        // not sit on the per-step dependency chain.  GPT == 1 (one CTA per SM, registers to spare): step s+1's values are
-        // requested at the top of step s and consumed a whole step later.  GPT == 2 (two CTAs per SM, register-tight): the
-        // loads stay at the top of their own step, but step s+1's lines are pulled into L2 a step ahead.
-        constexpr bool kRegPrefetch = (GPT == 1);
-        // (kept in the storage type: converting an FP16 value at load time would make the load's result a dependency of the
-        // same step and forfeit the step of latency hiding)
-        TG gn[kRegPrefetch ? NM : 1][kRegPrefetch ? kNS : 1];
-        const TG* const bptr_g = nullptr;
-        (void)bptr_g;
-        if (kRegPrefetch) {
+        for (int j = 0; j < kItems; ++j) {
+            c_state[j][0] = c_state[j][1] = 0.f;
+            if (ok[j] && (unsigned)(0 - g_lo) < (unsigned)g_len) {
 #pragma unroll
-            for (int i = 0; i < kNS; ++i) {
-                const bool real = (unsigned)(0 - g_lo[i]) < (unsigned)g_len[i];
-#pragma unroll
-                for (int m = 0; m < NM; ++m) gn[kRegPrefetch ? m : 0][kRegPrefetch ? i : 0] = real ? gin[goff[i] + m * gtile] : to_storage<TG>(bptr[m * gtile]);
-                goff[i] += gstep;
+                for (int q = 0; q < 4; ++q) gn[j][q] = *reinterpret_cast<const TG2*>(gin + goff + cstep * j + q * H);
             }
         }
+        goff += gstep;
         for (int s = 0; s < p.steps; ++s) {
-            float gi[NM][kNS];
-            if (kRegPrefetch) {
+            float2 gi[kItems][4];
+            const bool real = (unsigned)(s - g_lo) < (unsigned)g_len;
+            const bool real_next = s + 1 < p.steps && (unsigned)(s + 1 - g_lo) < (unsigned)g_len;
+            const bool real_next2 = s + 2 < p.steps && (unsigned)(s + 2 - g_lo) < (unsigned)g_len;
 #pragma unroll
-                for (int i = 0; i < kNS; ++i) {
+            for (int j = 0; j < kItems; ++j) {
+                if (!ok[j]) continue;
 #pragma unroll
-                    for (int m = 0; m < NM; ++m) gi[m][i] = ldf(&gn[kRegPrefetch ? m : 0][kRegPrefetch ? i : 0]);
+                for (int q = 0; q < 4; ++q) gi[j][q] = real ? to_f2(gn[j][q]) : ld2f(bias_pad + gcol + cstep * j + q * H);
+                if (real_next) {
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) gn[j][q] = *reinterpret_cast<const TG2*>(gin + goff + cstep * j + q * H);
                 }
-                if (s + 1 < p.steps) {
+                // and the step after that into L2: a register load a single step ahead does not cover HBM latency under load
+                if (real_next2) {
 #pragma unroll
-                    for (int i = 0; i < kNS; ++i) {
-                        const bool real = (unsigned)(s + 1 - g_lo[i]) < (unsigned)g_len[i];
-#pragma unroll
-                        for (int m = 0; m < NM; ++m) gn[kRegPrefetch ? m : 0][kRegPrefetch ? i : 0] = real ? gin[goff[i] + m * gtile] : to_storage<TG>(bptr[m * gtile]);
-                        goff[i] += gstep;
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < kNS; ++i) {
-                    const bool real = (unsigned)(s - g_lo[i]) < (unsigned)g_len[i];
-#pragma unroll
-                    for (int m = 0; m < NM; ++m) gi[m][i] = real ? ldf(gin + goff[i] + m * gtile) : bptr[m * gtile];
-                    goff[i] += gstep;
+                    for (int q = 0; q < 4; ++q)
+                        asm volatile("prefetch.global.L2 [%0];" ::"l"(gin + goff + gstep + cstep * j + q * H));
                 }
             }
-            if (ew == 0 && lane == 0) LSTM_TRACE(2, s);
-            if (s > 0) {
-                mbar_wait(&sh->acc_ready, (uint32_t)((s - 1) & 1));
+            goff += gstep;
+            if (g == 0 && t == 0) LSTM_TRACE(2, s);
+            if (s > 0) mbar_wait(&sh->acc_ready[g], (uint32_t)((s - 1) & 1));
+            if (g == 0 && t == 0) LSTM_TRACE(3, s);
+            const bool store = (unsigned)(s - w_lo) < (unsigned)w_len;
+#pragma unroll
+            for (int j = 0; j < kItems; ++j) {
+                if (!ok[j]) continue;
+                float act[4][2];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const float2 acc = s > 0 ? *reinterpret_cast<const float2*>(accn + cstep * j + q * H) : make_float2(0.f, 0.f);
+                    // PyTorch gate order 0 i, 1 f, 2 g, 3 o; gate 2 is tanh = 2*sigmoid(2x) - 1: fold into scale / affine
+                    const float k_in = (q == 2) ? -2.885390081777927f : -1.4426950408889634f;   // -(1|2) * log2(e)
+                    const float k_mul = (q == 2) ? 2.0f : 1.0f, k_add = (q == 2) ? -1.0f : 0.0f;
+                    act[q][0] = fmaf(k_mul, fast_rcp(1.0f + fast_ex2(k_in * (acc.x + gi[j][q].x))), k_add);
+                    act[q][1] = fmaf(k_mul, fast_rcp(1.0f + fast_ex2(k_in * (acc.y + gi[j][q].y))), k_add);
+                }
+                float h[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float c = fmaf(act[1][e], c_state[j][e], act[0][e] * act[2][e]);
+                    c_state[j][e] = c;
+                    const float th = fmaf(2.0f, fast_rcp(1.0f + fast_ex2(-2.885390081777927f * c)), -1.0f);
+                    h[e] = round_tf32_rna(act[3][e] * th);
+                }
+                const __half2 hh = __floats2half2_rn(h[0], h[1]);
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(baddr[j]), "r"(*reinterpret_cast<const uint32_t*>(&hh)) : "memory");
+                if (store) st2(hout + ooff + cstep * j, h[0], h[1]);
             }
-            if (ew == 0 && lane == 0) LSTM_TRACE(3, s);
-            float a[NM][kNS];
-#pragma unroll
-            for (int m = 0; m < NM; ++m) {
-                uint32_t acc[kNS];
-                if (s > 0) {
-                    const uint32_t arow = smem_u32(sAcc + (m * 128 + r) * kLdAcc + wp * kNS);
-#pragma unroll
-                    for (int i = 0; i < kNS; i += 4) {
-                        const float4 v = lds128(arow + 4u * i);
-                        acc[i] = __float_as_uint(v.x); acc[i + 1] = __float_as_uint(v.y); acc[i + 2] = __float_as_uint(v.z); acc[i + 3] = __float_as_uint(v.w);
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < kNS; ++i) acc[i] = 0u;
-                }
-                // PyTorch gate order 0 i, 1 f, 2 g, 3 o; gate 2 is tanh = 2*sigmoid(2x) - 1: fold into scale / affine
-                const int gate = m * GPT + sub;
-                const float k_in = (gate == 2) ? -2.885390081777927f : -1.4426950408889634f;   // -(1|2) * log2(e)
-                const float k_mul = (gate == 2) ? 2.0f : 1.0f, k_add = (gate == 2) ? -1.0f : 0.0f;
-#pragma unroll
-                for (int i = 0; i < kNS; ++i) {
-                    const float x = __uint_as_float(acc[i]) + gi[m][i];
-                    a[m][i] = fmaf(k_mul, fast_rcp(1.0f + fast_ex2(k_in * x)), k_add);
-                }
-            }
-            if (ew == 0 && lane == 0) LSTM_TRACE(4, s);
-#pragma unroll
-            for (int ii = 0; ii < kMS; ++ii) {
-                float ig, fg, gg, og;
-                if (GPT == 1) {
-                    ig = a[0][ii]; fg = a[1 % NM][ii]; gg = a[2 % NM][ii]; og = a[3 % NM][ii];
-                } else {
-                    // this lane finishes sequence 2*ii + sub and hands its two gates of sequence 2*ii + (1 - sub) to the partner
-                    const int e = (2 * ii) % kNS, o = (2 * ii + 1) % kNS;
-                    const float own0 = sub ? a[0][o] : a[0][e], own1 = sub ? a[1 % NM][o] : a[1 % NM][e];
-                    const float snd0 = sub ? a[0][e] : a[0][o], snd1 = sub ? a[1 % NM][e] : a[1 % NM][o];
-                    const float p0 = __shfl_xor_sync(0xffffffffu, snd0, 16);
-                    const float p1 = __shfl_xor_sync(0xffffffffu, snd1, 16);
-                    if (sub == 0) { ig = own0; gg = own1; fg = p0; og = p1; }
-                    else          { fg = own0; og = own1; ig = p0; gg = p1; }
-                }
-                const float c = fmaf(fg, c_state[ii], ig * gg);
-                c_state[ii] = c;
-                const float th = fmaf(2.0f, fast_rcp(1.0f + fast_ex2(-2.885390081777927f * c)), -1.0f);
-                const float h = round_tf32_rna(og * th);
-                if (cell_ok) {
-                    const unsigned short hh = __half_as_ushort(__float2half_rn(h));
-                    asm volatile("st.shared.u16 [%0], %1;" ::"r"(baddr[ii]), "h"(hh) : "memory");
-                }
-                if ((unsigned)(s - w_lo[ii]) < (unsigned)w_len[ii]) stf(hout + ooff[ii], h);
-                ooff[ii] += ostep;
-            }
-            if (ew == 0 && lane == 0) LSTM_TRACE(5, s);
+            ooff += ostep;
+            if (g == 0 && t == 0) LSTM_TRACE(5, s);
             if (s + 1 < p.steps) {
                 fence_proxy_async_smem();                // generic-proxy stores of h -> visible to the tensor core
-                mbar_arrive(&sh->h_ready);
+                mbar_arrive(&sh->h_ready[g]);
             }
-            if (ew == 0 && lane == 0) LSTM_TRACE(6, s);
+            if (g == 0 && t == 0) LSTM_TRACE(6, s);
         }
     }
 }
 
-template <int GPT, int NEW, int SEQ, int ROWB, int MINB, typename TO>
-static void lstm_tc_go(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& mW, const void* gin, const float* bias_pad, void* hout,
-                       const aero_lstm_params& p, int nK) {
+template <int KS, int NT, typename TO>
+static void lstm_tc_go(dim3 grid, size_t smem, cudaStream_t st, const void* whh, const void* gin, const float* bias_pad, void* hout,
+                       const aero_lstm_params& p, const LstmTcShape& sp) {
+    const __half* w = static_cast<const __half*>(whh);
+    constexpr int kThreads = LstmTcCfg<KS>::kThreads;
     if (p.flags & AERO_TG_A_F16) {          // gate pre-activations stored in FP16
-        cudaFuncSetAttribute(lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, __half><<<grid, 128 + 32 * NEW, smem, st>>>(mW, static_cast<const __half*>(gin), bias_pad,
-                                                                                              static_cast<TO*>(hout), p, nK);
+        cudaFuncSetAttribute(lstm_tc_kernel<KS, NT, TO, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        lstm_tc_kernel<KS, NT, TO, __half><<<grid, kThreads, smem, st>>>(w, static_cast<const __half*>(gin), bias_pad,
+                                                                         static_cast<TO*>(hout), p, sp.S, sp.tps);
     } else {
-        cudaFuncSetAttribute(lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        lstm_tc_kernel<GPT, NEW, SEQ, ROWB, MINB, TO, float><<<grid, 128 + 32 * NEW, smem, st>>>(mW, static_cast<const float*>(gin), bias_pad,
-                                                                                             static_cast<TO*>(hout), p, nK);
+        cudaFuncSetAttribute(lstm_tc_kernel<KS, NT, TO, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        lstm_tc_kernel<KS, NT, TO, float><<<grid, kThreads, smem, st>>>(w, static_cast<const float*>(gin), bias_pad,
+                                                                        static_cast<TO*>(hout), p, sp.S, sp.tps);
     }
+}
+
+template <int KS>
+static void lstm_tc_dispatch(dim3 grid, cudaStream_t st, const void* whh, const void* gin, const float* bias_pad, void* hout,
+                             const aero_lstm_params& p, const LstmTcShape& sp) {
+    const size_t smem = 1024 + 2 * (size_t)((KS + 3) / 4) * sp.nt * 128 + 2 * (size_t)sp.nt * LstmTcCfg<KS>::kLdr * 4 + sizeof(LstmTcShared);
+    const bool o16 = p.flags & AERO_TG_OUT_F16;
+    constexpr int kWide = KS == 6 ? 8 : 16;      // lstm_tc_shape never picks N = 16 at KS = 6
+    if (sp.nt == 8) {
+        if (o16) lstm_tc_go<KS, 8, __half>(grid, smem, st, whh, gin, bias_pad, hout, p, sp);
+        else lstm_tc_go<KS, 8, float>(grid, smem, st, whh, gin, bias_pad, hout, p, sp);
+    } else {
+        if (o16) lstm_tc_go<KS, kWide, __half>(grid, smem, st, whh, gin, bias_pad, hout, p, sp);
+        else lstm_tc_go<KS, kWide, float>(grid, smem, st, whh, gin, bias_pad, hout, p, sp);
+    }
+}
+
+// Launch shape.  A CTA holds W_hh once (registers of its MMA warpgroups) and two groups of S sequences of one direction, one CTA
+// per SM.  A sequence takes tps = ceil((H / 2) / kItems) cell threads, so a group of 128 holds at most 128 / tps sequences
+// (8 at H = 96, 16 at H = 48).  S is the smallest width that puts every CTA of both directions on the GPU in one wave,
+// ceil(n_seq / (2 floor(sms / 2))), capped there and at 16 (8 for H > 80); beyond the cap the grid takes more than one wave.
+// wgmma N = 8 for S <= 8, else 16.
+LstmTcShape lstm_tc_shape(int n_seq, int H, int num_sms) {
+    LstmTcShape r;
+    r.tps = cdiv(H / 2, kItems);
+    const int per_dir = std::max(1, num_sms / 2);
+    // two MMA warpgroups (H > 80) leave 128 registers per thread: wgmma N = 16 would spill there, so S <= 8
+    const int cap = std::min((H + 15) / 16 == 6 ? 8 : 16, kCellThreads / r.tps);
+    r.S = std::max(1, std::min(cap, cdiv(n_seq, 2 * per_dir)));
+    r.nt = r.S <= 8 ? 8 : 16;
+    r.ctas_per_dir = cdiv(n_seq, 2 * r.S);
+    return r;
 }
 
 int lstm_tc_launch(const void* gin, const float* bias_pad, const void* whh_r, void* hout, const aero_lstm_params& p,
                    cudaStream_t st) {
     const int H = p.H;
-    if (H % 4 || H <= 32 || H > 128) {
-        set_error("aero_lstm_rec_fwd(wgmma): hidden size %d unsupported (multiple of 4 in (32, 128])", H);
+    if (H % 4 || H <= 32 || H > 96) {
+        set_error("aero_lstm_rec_fwd(wgmma): hidden size %d unsupported (multiple of 4 in (32, 96])", H);
         return AERO_ERR_UNSUPPORTED;
     }
     static int num_sms = 0;
@@ -370,49 +346,30 @@ int lstm_tc_launch(const void* gin, const float* bias_pad, const void* whh_r, vo
         cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
     }
     const int n_seq = p.rows * p.n_win;
-    const int gpt = H <= 64 ? 2 : 1;
-    const int nM = 4 / gpt;
-    const int Kp = ((H + 63) / 64) * 64;                 // the host pads W_hh rows to a multiple of 64 fp16 (128 bytes)
-    // Small CTAs (8 sequences) whenever all of them fit on the GPU at once at the co-residency they allow: twice the SMs
-    // busy and, where two share an SM (GPT = 2), one CTA's barrier / MMA latency hides behind another's cell update.
-    // GPT = 1 keeps W_hh in 32-column SWIZZLE_64B chunks then (no K padding).
-    const int knob = lstm_seq_knob();
-    const bool small = knob ? knob == 8 : (int64_t)cdiv(n_seq, 8) * 2 <= (int64_t)num_sms * (gpt == 1 ? 1 : 2);
-    const int rowb = (gpt == 1 && small) ? 64 : 128;
-    const int kc_elems = rowb / 2;
-    const int nK = (H + kc_elems - 1) / kc_elems;
-    CUtensorMap mW;
-    uint64_t dims[2] = {(uint64_t)Kp, (uint64_t)(2 * nM * 128)};
-    uint64_t strides[1] = {(uint64_t)Kp * 2};
-    uint32_t box[2] = {(uint32_t)kc_elems, 128};
-    int rc = encode_map(&mW, whh_r, 2, dims, strides, box, rowb == 64 ? 2 : 0, 2);
-    if (rc != AERO_OK) return rc;
-    const size_t smem = (size_t)nM * nK * 128 * rowb + (size_t)nK * kNT * rowb + (size_t)nM * 128 * kLdAcc * 4 + sizeof(LstmTcShared) + 1024;
-    if (smem > 227 * 1024) {
-        set_error("aero_lstm_rec_fwd(wgmma): hidden size %d needs %zu bytes of shared memory", H, smem);
-        return AERO_ERR_UNSUPPORTED;
-    }
+    const LstmTcShape sp = lstm_tc_shape(n_seq, H, num_sms);
     const int64_t max_rows = (int64_t)n_seq * p.steps > (int64_t)p.rows * p.T ? (int64_t)n_seq * p.steps : (int64_t)p.rows * p.T;
     if ((max_rows + p.steps) * (8ll * H) >= (1ll << 31)) {
         set_error("aero_lstm_rec_fwd(wgmma): problem too large for 32-bit offsets (%lld rows)", (long long)max_rows);
         return AERO_ERR_UNSUPPORTED;
     }
-    dim3 grid(cdiv(n_seq, small ? 8 : kNT), 2);
-    const bool o16 = p.flags & AERO_TG_OUT_F16;
-#define AERO_LSTM_GO(GPT, NEW, SEQ, ROWB, MINB)                                                              \
-    do {                                                                                                      \
-        if (o16) lstm_tc_go<GPT, NEW, SEQ, ROWB, MINB, __half>(grid, smem, st, mW, gin, bias_pad, hout, p, nK); \
-        else lstm_tc_go<GPT, NEW, SEQ, ROWB, MINB, float>(grid, smem, st, mW, gin, bias_pad, hout, p, nK);      \
-    } while (0)
-    if (gpt == 1) {
-        if (small) AERO_LSTM_GO(1, 8, 8, 64, 1);
-        else AERO_LSTM_GO(1, 16, 16, 128, 1);
-    } else {
-        if (small) AERO_LSTM_GO(2, 8, 8, 128, 2);
-        else AERO_LSTM_GO(2, 8, 16, 128, 2);
+    const dim3 grid(sp.ctas_per_dir, 2);
+    switch ((H + 15) / 16) {
+        case 3: lstm_tc_dispatch<3>(grid, st, whh_r, gin, bias_pad, hout, p, sp); break;
+        case 4: lstm_tc_dispatch<4>(grid, st, whh_r, gin, bias_pad, hout, p, sp); break;
+        case 5: lstm_tc_dispatch<5>(grid, st, whh_r, gin, bias_pad, hout, p, sp); break;
+        default: lstm_tc_dispatch<6>(grid, st, whh_r, gin, bias_pad, hout, p, sp); break;
     }
-#undef AERO_LSTM_GO
     return check_launch("aero_lstm_rec_fwd(wgmma)");
 }
 
 }  // namespace aero
+
+extern "C" int aero_lstm_tc_shape(int32_t n_seq, int32_t H, int32_t num_sms, int32_t* out) {
+    if (!out || n_seq < 1 || H % 4 || H <= 32 || H > 96 || num_sms < 1) return AERO_ERR_INVALID;
+    const aero::LstmTcShape r = aero::lstm_tc_shape(n_seq, H, num_sms);
+    out[0] = r.S;
+    out[1] = r.nt;
+    out[2] = r.ctas_per_dir;
+    out[3] = r.tps;
+    return AERO_OK;
+}

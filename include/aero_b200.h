@@ -262,6 +262,9 @@ typedef struct {
 } aero_lstm_params;
 int aero_lstm_rec_fwd(const void* gin, const float* bias_pad, const void* whh, void* hout,
                       const aero_lstm_params* p, aero_stream_t stream);
+/* Launch shape of the wgmma recurrence (precision 1) for n_seq = rows * n_win sequences on num_sms SMs: out[0] = sequences per
+ * group (two groups per CTA), out[1] = wgmma N (8 or 16), out[2] = CTAs per direction, out[3] = cell-update threads per sequence.  AERO_ERR_INVALID outside the supported H. */
+int aero_lstm_tc_shape(int32_t n_seq, int32_t H, int32_t num_sms, int32_t* out);
 
 /* ------------------------------------------------------------------------------------------
  * LocalState attention core (replaces the einsum/softmax/einsum chain reference
