@@ -141,6 +141,14 @@ SYMBOLS = {
     # GAN loss terms
     "aero_gan_loss_fwd": (C.c_int, [vp, i32, vp, vp, vp]),
     "aero_gan_loss_bwd": (C.c_int, [vp, i32, vp]),
+    # ragged batches (clips of different lengths in one forward)
+    "aero_stft_varlen_fwd": (C.c_int, [vp, vp, vp, vp, vp, C.POINTER(StftParams), vp]),
+    "aero_istft_varlen_fwd": (C.c_int, [vp, vp, vp, vp, vp, C.POINTER(IstftParams), vp]),
+    "aero_sample_norm_varlen_fwd": (C.c_int, [vp, vp, vp, vp, vp, i32, i64, i64, i32, vp]),
+    "aero_masked_stats_fwd": (C.c_int, [vp, vp, vp] + [i32] * 7 + [vp]),
+    "aero_frame_mask_fwd": (C.c_int, [vp, vp] + [i32] * 5 + [vp]),
+    "aero_gather_rows_fwd": (C.c_int, [vp, vp, vp, vp, i64, i32, i32, i32, vp]),
+    "aero_local_attn_varlen_fwd": (C.c_int, [vp, vp, vp, i32, C.POINTER(AttnParams), vp]),
 }
 
 

@@ -8,15 +8,16 @@ namespace aero {
 constexpr int kQB = 128;     // queries per CTA (one per thread)
 constexpr int kKT = 256;     // keys per shared-memory tile
 
+// Rows are p.T frames apart; the first Tr of them take part (Tr = p.T, or the row's own length in a ragged batch).
 template <int D, typename TO>
-__global__ void __launch_bounds__(kQB) local_attn_kernel(const float* __restrict__ qkvd, TO* __restrict__ out,
-                                                         const aero_attn_params p) {
+__device__ __forceinline__ void local_attn_block(const float* __restrict__ qkvd, TO* __restrict__ out,
+                                                 const aero_attn_params& p, const int Tr) {
     __shared__ __align__(16) float Ks[kKT * D];
     __shared__ __align__(16) float Vs[kKT * D];
     const int row = blockIdx.z, h = blockIdx.y;
     const int s = blockIdx.x * kQB + threadIdx.x;
-    const bool valid = s < p.T;
-    const int sq = valid ? s : p.T - 1;
+    const bool valid = s < Tr;
+    const int sq = valid ? s : Tr - 1;
     const float* base = qkvd + (int64_t)row * p.T * p.ld;
 
     float q[D];
@@ -32,8 +33,8 @@ __global__ void __launch_bounds__(kQB) local_attn_kernel(const float* __restrict
 #pragma unroll
     for (int c = 0; c < D; ++c) acc[c] = 0.f;
 
-    for (int k0 = 0; k0 < p.T; k0 += kKT) {
-        const int nk = min(kKT, p.T - k0);
+    for (int k0 = 0; k0 < Tr; k0 += kKT) {
+        const int nk = min(kKT, Tr - k0);
         __syncthreads();
         for (int i = threadIdx.x; i < nk * D; i += kQB) {
             const int t = i / D, c = i - t * D;
@@ -87,6 +88,22 @@ __global__ void __launch_bounds__(kQB) local_attn_kernel(const float* __restrict
     }
 }
 
+template <int D, typename TO>
+__global__ void __launch_bounds__(kQB) local_attn_kernel(const float* __restrict__ qkvd, TO* __restrict__ out,
+                                                         const aero_attn_params p) {
+    local_attn_block<D, TO>(qkvd, out, p, p.T);
+}
+
+// ragged batch: row r belongs to clip r / rows_per_clip, whose first frames[clip] frames are valid
+template <int D, typename TO>
+__global__ void __launch_bounds__(kQB) local_attn_varlen_kernel(const float* __restrict__ qkvd, TO* __restrict__ out,
+                                                                const int32_t* __restrict__ frames, const int rows_per_clip,
+                                                                const aero_attn_params p) {
+    const int Tr = frames[blockIdx.z / rows_per_clip];
+    if ((int)blockIdx.x * kQB >= Tr) return;
+    local_attn_block<D, TO>(qkvd, out, p, Tr);
+}
+
 template <int D>
 static int launch_attn(const float* qkvd, void* out, const aero_attn_params& p, cudaStream_t st) {
     dim3 grid(cdiv(p.T, kQB), p.heads, p.rows);
@@ -95,7 +112,19 @@ static int launch_attn(const float* qkvd, void* out, const aero_attn_params& p, 
     return check_launch("aero_local_attn_fwd");
 }
 
-int local_attn_mma_launch(const float* qkvd, void* out, const aero_attn_params& p, cudaStream_t st, bool* taken);
+template <int D>
+static int launch_attn_varlen(const float* qkvd, void* out, const int32_t* frames, int rows_per_clip, const aero_attn_params& p,
+                              cudaStream_t st) {
+    dim3 grid(cdiv(p.T, kQB), p.heads, p.rows);
+    if (p.flags & AERO_TG_OUT_F16)
+        local_attn_varlen_kernel<D, __half><<<grid, kQB, 0, st>>>(qkvd, static_cast<__half*>(out), frames, rows_per_clip, p);
+    else
+        local_attn_varlen_kernel<D, float><<<grid, kQB, 0, st>>>(qkvd, static_cast<float*>(out), frames, rows_per_clip, p);
+    return check_launch("aero_local_attn_varlen_fwd");
+}
+
+int local_attn_mma_launch(const float* qkvd, void* out, const aero_attn_params& p, cudaStream_t st, bool* taken,
+                          const int32_t* frames, int rows_per_clip);
 }  // namespace aero
 
 extern "C" int aero_local_attn_fwd(const float* qkvd, void* out, const aero_attn_params* p, aero_stream_t stream) {
@@ -107,7 +136,7 @@ extern "C" int aero_local_attn_fwd(const float* qkvd, void* out, const aero_attn
     cudaStream_t st = (cudaStream_t)stream;
     if (p->flags & AERO_TG_ROUND_TF32) {            // tensor-core mode: TF32 mma.sync kernel (attention_mma.cu)
         bool taken = false;
-        const int rc = local_attn_mma_launch(qkvd, out, *p, st, &taken);
+        const int rc = local_attn_mma_launch(qkvd, out, *p, st, &taken, nullptr, 0);
         if (taken || rc != AERO_OK) return rc;
     }
     switch (p->H / p->heads) {
@@ -117,6 +146,31 @@ extern "C" int aero_local_attn_fwd(const float* qkvd, void* out, const aero_attn
         case 24: return launch_attn<24>(qkvd, out, *p, st);
         default:
             set_error("aero_local_attn_fwd: head dim %d not instantiated (3, 6, 12, 24)", p->H / p->heads);
+            return AERO_ERR_UNSUPPORTED;
+    }
+}
+
+extern "C" int aero_local_attn_varlen_fwd(const float* qkvd, void* out, const int32_t* frames, int32_t rows_per_clip,
+                                          const aero_attn_params* p, aero_stream_t stream) {
+    using namespace aero;
+    AERO_REQUIRE(qkvd && out && frames && p, "aero_local_attn_varlen_fwd: null argument");
+    AERO_REQUIRE(p->heads >= 1 && p->H % p->heads == 0 && p->ndecay >= 1 && p->ndecay <= 16, "aero_local_attn_varlen_fwd: heads/ndecay");
+    AERO_REQUIRE(p->ld >= 3 * p->H + p->heads * p->ndecay, "aero_local_attn_varlen_fwd: ld=%d too small", p->ld);
+    AERO_REQUIRE(p->rows >= 1 && p->rows <= 65535 && p->T >= 1, "aero_local_attn_varlen_fwd: rows=%d", p->rows);
+    AERO_REQUIRE(rows_per_clip >= 1 && p->rows % rows_per_clip == 0, "aero_local_attn_varlen_fwd: rows_per_clip=%d", rows_per_clip);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (p->flags & AERO_TG_ROUND_TF32) {
+        bool taken = false;
+        const int rc = local_attn_mma_launch(qkvd, out, *p, st, &taken, frames, rows_per_clip);
+        if (taken || rc != AERO_OK) return rc;
+    }
+    switch (p->H / p->heads) {
+        case 3: return launch_attn_varlen<3>(qkvd, out, frames, rows_per_clip, *p, st);
+        case 6: return launch_attn_varlen<6>(qkvd, out, frames, rows_per_clip, *p, st);
+        case 12: return launch_attn_varlen<12>(qkvd, out, frames, rows_per_clip, *p, st);
+        case 24: return launch_attn_varlen<24>(qkvd, out, frames, rows_per_clip, *p, st);
+        default:
+            set_error("aero_local_attn_varlen_fwd: head dim %d not instantiated (3, 6, 12, 24)", p->H / p->heads);
             return AERO_ERR_UNSUPPORTED;
     }
 }

@@ -31,9 +31,10 @@ __device__ __forceinline__ float ex2f(float x) {
     return y;
 }
 
+// Rows are p.T frames apart; the first Tr of them take part (Tr = p.T, or the row's own length in a ragged batch).
 template <int D, typename TO>   // head dim: 12 or 24
-__global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __restrict__ qkvd, TO* __restrict__ out,
-                                                             const aero_attn_params p) {
+__device__ __forceinline__ void local_attn_mma_block(const float* __restrict__ qkvd, TO* __restrict__ out,
+                                                     const aero_attn_params& p, const int Tr) {
     constexpr int DP = (D + 7) / 8 * 8;                  // 16 or 24
     constexpr int KS = DP / 8;                           // k-steps of QK^T == n-tiles of PV
     constexpr int PITCH = DP + 4;                        // 20 / 28: conflict-free fragment loads
@@ -51,7 +52,7 @@ __global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __rest
 
     // ---- Q fragments (A operand), rows g / g+8, pre-scaled so that scores come out in the log2 domain
     const int s_lo = q0 + g, s_hi = q0 + g + 8;
-    const int sl = min(s_lo, p.T - 1), sh = min(s_hi, p.T - 1);
+    const int sl = min(s_lo, Tr - 1), sh = min(s_hi, Tr - 1);
     const float qs = kLog2e * rsqrtf((float)D);
     uint32_t qa[KS][4];
 #pragma unroll
@@ -83,8 +84,8 @@ __global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __rest
         for (int i = threadIdx.x; i < kAKT * CH * 2; i += 128) {
             const int which = i / (kAKT * CH), j = i - which * (kAKT * CH);
             const int t = j / CH, c4 = j - t * CH;
-            const bool ok = k0 + t < p.T;
-            const float* src = base + (int64_t)min(k0 + t, p.T - 1) * p.ld + (which + 1) * p.H + h * D + 4 * c4;
+            const bool ok = k0 + t < Tr;
+            const float* src = base + (int64_t)min(k0 + t, Tr - 1) * p.ld + (which + 1) * p.H + h * D + 4 * c4;
             const uint32_t dst = (uint32_t)__cvta_generic_to_shared((which ? &Vsm[buf][0] : &Ksm[buf][0]) + t * PITCH + 4 * c4);
             asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
         }
@@ -92,9 +93,9 @@ __global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __rest
     };
     fill(0, 0);
     int it = 0;
-    for (int k0 = 0; k0 < p.T; k0 += kAKT, ++it) {
-        const int nk = min(kAKT, p.T - k0);
-        if (k0 + kAKT < p.T) fill(k0 + kAKT, (it + 1) & 1);
+    for (int k0 = 0; k0 < Tr; k0 += kAKT, ++it) {
+        const int nk = min(kAKT, Tr - k0);
+        if (k0 + kAKT < Tr) fill(k0 + kAKT, (it + 1) & 1);
         else asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 1;" ::: "memory");
         __syncthreads();
@@ -130,9 +131,9 @@ __global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __rest
                         if (t_a == s_hi) sc[u][2] = kDiag;
                         if (t_a + 1 == s_hi) sc[u][3] = kDiag;
                     }
-                    if (kb0 + 8 > p.T) {                                               // padding keys of the last block
-                        if (t_a >= p.T) { sc[u][0] = -1e30f; sc[u][2] = -1e30f; }
-                        if (t_a + 1 >= p.T) { sc[u][1] = -1e30f; sc[u][3] = -1e30f; }
+                    if (kb0 + 8 > Tr) {                                               // padding keys of the last block
+                        if (t_a >= Tr) { sc[u][0] = -1e30f; sc[u][2] = -1e30f; }
+                        if (t_a + 1 >= Tr) { sc[u][1] = -1e30f; sc[u][3] = -1e30f; }
                     }
                     cm_lo = fmaxf(cm_lo, fmaxf(sc[u][0], sc[u][1]));
                     cm_hi = fmaxf(cm_hi, fmaxf(sc[u][2], sc[u][3]));
@@ -179,12 +180,12 @@ __global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __rest
     for (int nt = 0; nt < KS; ++nt) {
         const int c = nt * 8 + 2 * tig;
         if (c < D) {
-            if (s_lo < p.T) {
+            if (s_lo < Tr) {
                 TO* op = out + ((int64_t)row * p.T + s_lo) * p.H + h * D + c;
                 stf(op, round_tf32_rna(o[nt][0] * il_lo));
                 if (c + 1 < D) stf(op + 1, round_tf32_rna(o[nt][1] * il_lo));
             }
-            if (s_hi < p.T) {
+            if (s_hi < Tr) {
                 TO* op = out + ((int64_t)row * p.T + s_hi) * p.H + h * D + c;
                 stf(op, round_tf32_rna(o[nt][2] * il_hi));
                 if (c + 1 < D) stf(op + 1, round_tf32_rna(o[nt][3] * il_hi));
@@ -193,11 +194,39 @@ __global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __rest
     }
 }
 
-int local_attn_mma_launch(const float* qkvd, void* out, const aero_attn_params& p, cudaStream_t st, bool* taken) {
+template <int D, typename TO>
+__global__ void __launch_bounds__(128) local_attn_mma_kernel(const float* __restrict__ qkvd, TO* __restrict__ out,
+                                                             const aero_attn_params p) {
+    local_attn_mma_block<D, TO>(qkvd, out, p, p.T);
+}
+
+// ragged batch: row r belongs to clip r / rows_per_clip, whose first frames[clip] frames are valid
+template <int D, typename TO>
+__global__ void __launch_bounds__(128) local_attn_mma_varlen_kernel(const float* __restrict__ qkvd, TO* __restrict__ out,
+                                                                    const int32_t* __restrict__ frames, const int rows_per_clip,
+                                                                    const aero_attn_params p) {
+    const int Tr = frames[blockIdx.z / rows_per_clip];
+    if ((int)blockIdx.x * kAQ >= Tr) return;
+    local_attn_mma_block<D, TO>(qkvd, out, p, Tr);
+}
+
+// frames != nullptr: ragged batch (aero_local_attn_varlen_fwd)
+int local_attn_mma_launch(const float* qkvd, void* out, const aero_attn_params& p, cudaStream_t st, bool* taken,
+                          const int32_t* frames, int rows_per_clip) {
     const int d = p.H / p.heads;
     *taken = (d == 12 || d == 24) && p.ld % 4 == 0 && p.H % 4 == 0 && (reinterpret_cast<uintptr_t>(qkvd) & 15) == 0;   // 16-byte cp.async chunks
     if (!*taken) return AERO_OK;
     dim3 grid(cdiv(p.T, kAQ), p.heads, p.rows);
+    if (frames) {
+        if (p.flags & AERO_TG_OUT_F16) {
+            if (d == 12) local_attn_mma_varlen_kernel<12, __half><<<grid, 128, 0, st>>>(qkvd, static_cast<__half*>(out), frames, rows_per_clip, p);
+            else local_attn_mma_varlen_kernel<24, __half><<<grid, 128, 0, st>>>(qkvd, static_cast<__half*>(out), frames, rows_per_clip, p);
+        } else {
+            if (d == 12) local_attn_mma_varlen_kernel<12, float><<<grid, 128, 0, st>>>(qkvd, static_cast<float*>(out), frames, rows_per_clip, p);
+            else local_attn_mma_varlen_kernel<24, float><<<grid, 128, 0, st>>>(qkvd, static_cast<float*>(out), frames, rows_per_clip, p);
+        }
+        return check_launch("aero_local_attn_varlen_fwd(mma)");
+    }
     if (p.flags & AERO_TG_OUT_F16) {
         if (d == 12) local_attn_mma_kernel<12, __half><<<grid, 128, 0, st>>>(qkvd, static_cast<__half*>(out), p);
         else local_attn_mma_kernel<24, __half><<<grid, 128, 0, st>>>(qkvd, static_cast<__half*>(out), p);

@@ -111,6 +111,82 @@ class _Stats:
         return view
 
 
+class _Ragged:
+    """Per-call state of a ragged batch (AeroEngine.forward_varlen): each clip's frame count on the host and as int32 device
+    tables, with its sample length and output length, and the BiLSTM framing tables built from them (one set per
+    (rows, T) key in `lstm_keys`).  Everything is built on the host first and uploaded in ONE asynchronous copy: a blocking
+    upload in the middle of the launch sequence would make the host wait for the device."""
+
+    def __init__(self, frames, device, lengths=None, out_lens=None, lstm_keys=()):
+        import numpy as np
+        self.frames = list(frames)
+        parts = [np.asarray(self.frames, np.int32), np.asarray(lengths or self.frames, np.int32),
+                 np.asarray(out_lens or self.frames, np.int32)]
+        meta = {}
+        for rows, T in lstm_keys:
+            n_seq, S, *tabs = lstm_ragged_tables(self.frames, rows // len(self.frames), T)
+            meta[(rows, T)] = (n_seq, S, [t_.shape for t_ in tabs])
+            parts += tabs
+        flat = torch.from_numpy(np.concatenate([p_.reshape(-1) for p_ in parts]))
+        if torch.device(device).type == "cuda":
+            flat = flat.pin_memory().to(device, non_blocking=True)
+        views, off = [], 0
+        for p_ in parts:
+            views.append(flat[off:off + p_.size].view(p_.shape))
+            off += p_.size
+        self.frames_d, self.lengths_d, self.out_lens_d = views[:3]
+        self.tables, i = {}, 3
+        for key, (n_seq, S, shapes) in meta.items():
+            self.tables[key] = (n_seq, S, *views[i:i + len(shapes)])
+            i += len(shapes)
+
+
+def lstm_ragged_tables(frames, F, T):
+    """Framing of reference modules.py:32-65 (BLSTM, max_steps 200) applied to each clip on its own, laid onto the windowed
+    layout [n_seq][S][..] of aero_lstm_rec_fwd, S = T if T <= 200 else 200.  Clip b (rows b*F .. b*F+F-1 of [rows][T]) is one
+    sequence of T_b steps if T_b <= 200, else ceil(T_b / 100) windows of 200 steps (stride 100).  A sequence of n < S steps
+    keeps its forward half at positions [0, n) and its reverse half at [S - n, S), so that the reverse recurrence starts at
+    the clip's own last step.  Returns (n_seq, S, index tables as int32 arrays of [rows, 2] for aero_gather_rows_fwd):
+      gin1 : layer-1 gate inputs from [rows*T] frames (-1: bias only, the reference's zero padding past T_b);
+      h1   : layer-1 outputs re-aligned to the real step of both halves (-1: zero);
+      gin2 : layer-2 gate inputs shifted back to the windowed layout (-1: bias);
+      out  : [rows*T] frames from the windowed layer-2 outputs with the reassembly crop (-1: zero, padded frames)."""
+    import numpy as np
+    S = T if T <= _LSTM_MAX_STEPS else _LSTM_MAX_STEPS
+    stride = _LSTM_MAX_STEPS // 2
+    half = stride // 2
+    gin1, h1, gin2, out = [], [], [], []
+    p = np.arange(S)
+    t = np.arange(T)
+    s0 = 0
+    for b, tb in enumerate(frames):
+        wins = [(0, tb)] if tb <= _LSTM_MAX_STEPS else [(k * stride, S) for k in range(-(-tb // stride))]
+        nw = len(wins)
+        # one row of this clip (row offset 0, sequences from 0), then all F rows by offsets
+        g1, a1, g2 = [], [], []
+        for k, (f0, n) in enumerate(wins):
+            q = p - (S - n)
+            g1.append(np.stack([np.where((p < n) & (f0 + p < tb), f0 + p, -1), np.where((q >= 0) & (f0 + q < tb), f0 + q, -1)], 1))
+            a1.append(np.stack([k * S + p, np.where(p < n, k * S + p + S - n, -1)], 1))
+            g2.append(np.stack([k * S + p, np.where(q >= 0, k * S + q, -1)], 1))
+        if nw == 1:
+            o = np.stack([t, t + S - wins[0][1]], 1)
+        else:
+            k = np.where(t < stride + half, 0, np.minimum((t - half) // stride, nw - 1))
+            o = np.repeat((k * S + t - k * stride)[:, None], 2, 1)
+        o = np.where((t < tb)[:, None], o, -1)
+        rows = np.arange(F)
+        seq_off = ((s0 + rows * nw) * S)[:, None, None]
+        shift = lambda v, off: np.where(v[None] >= 0, v[None] + off, -1).reshape(-1, 2)
+        gin1.append(shift(np.concatenate(g1), ((b * F + rows) * T)[:, None, None]))
+        h1.append(shift(np.concatenate(a1), seq_off))
+        gin2.append(shift(np.concatenate(g2), seq_off))
+        out.append(shift(o, seq_off))
+        s0 += F * nw
+    cat = lambda a: np.ascontiguousarray(np.concatenate(a).astype(np.int32))
+    return s0, S, cat(gin1), cat(h1), cat(gin2), cat(out)
+
+
 class AeroEngine:
     def __init__(self, model):
         self._init_state(model, cabi.load())
@@ -160,6 +236,7 @@ class AeroEngine:
         self.use_graph = "auto"
         self._graphs = {}
         self._seen = {}
+        self._vl = None             # _Ragged while forward_varlen runs
 
     # ------------------------------------------------------------------ plumbing
     def invalidate(self):
@@ -178,7 +255,7 @@ class AeroEngine:
             while len(self._bufsets) >= self.max_shape_sets:
                 old = next(iter(self._bufsets))
                 del self._bufsets[old]
-                for gk in [gk for gk in self._graphs if gk[0] == old[0] and gk[2] == old[1]]:
+                for gk in [gk for gk in self._graphs if len(old) == 2 and gk[0] == old[0] and gk[2] == old[1]]:
                     del self._graphs[gk]
         self._bufsets[key] = cur
         self._bufs = cur
@@ -484,7 +561,46 @@ class AeroEngine:
     def _attn(self, qkvd, out, *, rows, T, H, heads, ndecay, ld):
         p = cabi.AttnParams(rows, T, H, heads, ndecay, ld, (cabi.TG_ROUND_TF32 if self.precision >= 1 else 0) |
                             (cabi.TG_OUT_F16 if out.dtype == torch.float16 else 0))
+        if self._vl is not None:
+            cabi.check(self.lib.aero_local_attn_varlen_fwd(_ptr(qkvd), _ptr(out), _ptr(self._vl.frames_d),
+                                                           rows // len(self._vl.frames), C.byref(p), self._stream()), self.lib)
+            return
         cabi.check(self.lib.aero_local_attn_fwd(_ptr(qkvd), _ptr(out), C.byref(p), self._stream()), self.lib)
+
+    # ---- ragged batches (forward_varlen): per-clip lengths in self._vl.frames_d
+    def _frame_mask(self, x):
+        """Zeros on the padded frames of x [B, F, T, C]."""
+        B, F_, T, C_ = x.shape
+        cabi.check(self.lib.aero_frame_mask_fwd(_ptr(x), _ptr(self._vl.frames_d), B, F_, T, C_,
+                                                cabi.TG_OUT_F16 if x.dtype == torch.float16 else 0, self._stream()), self.lib)
+
+    def _masked_stats(self, x, stats, *, groups, scope):
+        """GroupNorm statistics of x [B, F, T, C] over each clip's valid frames, in the slots norm_act reads."""
+        B, F_, T, C_ = x.shape
+        cabi.check(self.lib.aero_masked_stats_fwd(_ptr(x), _ptr(stats), _ptr(self._vl.frames_d), B, F_, T, C_, groups, scope,
+                                                  cabi.TG_A_F16 if x.dtype == torch.float16 else 0, self._stream()), self.lib)
+
+    def _gather_rows(self, src, dst, idx, fill, n_rows):
+        cabi.check(self.lib.aero_gather_rows_fwd(_ptr(src), _ptr(dst), _ptr(idx), _ptr(fill), n_rows, dst.shape[-1], idx.shape[-1],
+                                                 cabi.TG_A_F16 if dst.dtype == torch.float16 else 0, self._stream()), self.lib)
+
+    def _sample_norm_varlen(self, x, stats, y, affine, B, per_frame, extent, rnd=False):
+        cabi.check(self.lib.aero_sample_norm_varlen_fwd(_ptr(x), _ptr(stats), _ptr(y), _ptr(affine), _ptr(self._vl.frames_d), B,
+                                                        per_frame, extent, 1 if rnd else 0, self._stream()), self.lib)
+
+    def _mask(self, x):
+        """Rule 2 of a ragged batch: a tensor that a time-coupled convolution reads holds zeros on padded frames."""
+        if self._vl is not None and x is not None:
+            self._frame_mask(x)
+
+    def _gemm_norm(self, raw, w, st, *, scope, groups, **kw):
+        """Tap-GEMM whose output feeds a GroupNorm.  Statistics come from the GEMM's epilogue, or, in a ragged batch (where the
+        epilogue would count padded frames), from a masked pass over the stored values."""
+        if self._vl is None:
+            return self._gemm(raw, w, stats=st, stats_mode=scope, groups=groups, **kw)
+        self._gemm(raw, w, groups=groups, **kw)
+        self._masked_stats(raw, st, groups=groups, scope=scope)
+        return raw
 
     def _sample_norm(self, x, stats, y, affine, B, per_sample, extent=None, rnd=False):
         cabi.check(self.lib.aero_sample_norm_fwd(_ptr(x), _ptr(stats), _ptr(y), _ptr(affine), B, per_sample,
@@ -515,6 +631,20 @@ class AeroEngine:
         frames = 1 + length // hop
         p = cabi.StftParams(n_fft, hop, win, n_sig, channels, length, frames, bins_out, *strides)
         rc = self.lib.aero_stft_fwd(_ptr(x), _ptr(self._window(win)), _ptr(z), _ptr(stats), C.byref(p), self._stream())
+        cabi.check(rc, self.lib)
+
+    def stft_varlen_into(self, x, lengths, z, stats, *, n_fft, hop, win, channels, bins_out, strides):
+        n_sig, length = x.shape[0], x.shape[1]
+        p = cabi.StftParams(n_fft, hop, win, n_sig, channels, length, 1 + length // hop, bins_out, *strides)
+        rc = self.lib.aero_stft_varlen_fwd(_ptr(x), _ptr(self._window(win)), _ptr(z), _ptr(stats), _ptr(lengths), C.byref(p),
+                                           self._stream())
+        cabi.check(rc, self.lib)
+
+    def istft_varlen_into(self, z, y, frames, out_lens, *, n_fft, hop, win, channels, frames_max, bins_in, strides):
+        n_sig, out_len = y.shape
+        p = cabi.IstftParams(n_fft, hop, win, n_sig, channels, frames_max, bins_in, out_len, *strides)
+        rc = self.lib.aero_istft_varlen_fwd(_ptr(z), _ptr(self._window(win)), _ptr(y), _ptr(frames), _ptr(out_lens), C.byref(p),
+                                            self._stream())
         cabi.check(rc, self.lib)
 
     def istft_into(self, z, y, *, n_fft, hop, win, channels, frames, bins_in, strides):
@@ -570,6 +700,7 @@ class AeroEngine:
         R = self._buf(tag + ".R", B, T, Fq * r, dtype=self._adt(Fq * r))
         self._gemm(R, W[p + ".ftb1.w"], a1=x, B=B, F_out=Fq, T=T, N=r, C1=Cc, bias=W[p + ".ftb1.b"], act=ACT_RELU,
                    o_s=(T * Fq * r, r, Fq * r), rnd=True)
+        self._mask(R.view(B, 1, T, Fq * r))          # the k=9 time convolution below reads it
         G = self._buf(tag + ".G", B, T, Cc)
         self._gemm(G, W[p + ".ftb1d.w"], a1=R, B=B, F_out=1, T=T, N=Cc, C1=Fq * r, kt=9, pad_t=4,
                    bias=W[p + ".ftb1d.b"], act=ACT_RELU, a1_s=(T * Fq * r, 0, Fq * r), o_s=(T * Cc, 0, Cc))
@@ -602,6 +733,7 @@ class AeroEngine:
         r = 5
         R = self._buf(tag + ".R", B, T, Fq * r, dtype=self._adt(Fq * r))
         self._ftb_lin_squeeze(xn, W[p + ".ftb1p.w"], W[p + ".ftb1p.b"], R, B=B, F=Fq, T=T, J=J, r=r, zrow=zrow)
+        self._mask(R.view(B, 1, T, Fq * r))
         G = self._buf(tag + ".G", B, T, Cc)
         self._gemm(G, W[p + ".ftb1d.w"], a1=R, B=B, F_out=1, T=T, N=Cc, C1=Fq * r, kt=9, pad_t=4,
                    bias=W[p + ".ftb1d.b"], act=ACT_RELU, a1_s=(T * Fq * r, 0, Fq * r), o_s=(T * Cc, 0, Cc))
@@ -620,6 +752,8 @@ class AeroEngine:
 
     def _blstm(self, h, W, o, rows, T, H, tag):
         """reference modules.py:32-65: framing, 2-layer BiLSTM, Linear, central-crop reassembly, skip."""
+        if self._vl is not None:
+            return self._blstm_ragged(h, W, o, rows, T, H, tag)
         if T > _LSTM_MAX_STEPS:
             steps, stride = _LSTM_MAX_STEPS, _LSTM_MAX_STEPS // 2
             n_win = math.ceil(T / stride)
@@ -642,6 +776,42 @@ class AeroEngine:
         h2 = self._buf(tag + ".h2", rows * T, 2 * H, dtype=self._adt(2 * H))
         self._lstm_rec(gin2, W[f"{o}.lstm1.b"], whh1, h2, rows=rows, T=T, H=H, n_win=n_win, steps=steps,
                        stride=stride, in_windowed=1, out_windowed=0, tc=tc)
+        self._gemm_flat(h, h2, W[o + ".lin.w"], rows * T, 2 * H, H, bias=W[o + ".lin.b"], residual=h, rnd=True)
+        return h
+
+    def _blstm_ragged(self, h, W, o, rows, T, H, tag):
+        """_blstm with each clip framed by its own length (lstm_ragged_tables): the gate inputs, the layer-1 outputs and the
+        final outputs pass through row gathers; both recurrences run on the windowed layout."""
+        vl = self._vl
+        key = (rows, T)
+        if key not in vl.tables:         # (forward_varlen builds every layer's tables up front; this covers direct use)
+            n_seq, S, *tabs = lstm_ragged_tables(vl.frames, rows // len(vl.frames), T)
+            vl.tables[key] = (n_seq, S, *(torch.from_numpy(t_).to(h.device) for t_ in tabs))
+        n_seq, S, i_gin1, i_h1, i_gin2, i_out = vl.tables[key]
+        # workspaces sized for the most sequences T frames can give, so that the shape set does not depend on the lengths
+        cap = (rows * math.ceil(T / (_LSTM_MAX_STEPS // 2)) if T > _LSTM_MAX_STEPS else rows) * S
+        n = n_seq * S
+        tc = self.lstm_tc and self.precision >= 1 and H % 4 == 0 and 32 < H <= 96
+        G = 8 * H
+        whh0, whh1 = (W[f"{o}.lstm0r.whh"], W[f"{o}.lstm1r.whh"]) if tc else (W[f"{o}.lstm0.whh"], W[f"{o}.lstm1.whh"])
+        gdt = torch.float16 if (tc and self.precision == 2 and self.gin16 and h.dtype == torch.float16) else torch.float32
+        gin = self._buf(tag + ".gin1", rows * T, G, dtype=gdt)
+        self._gemm_flat(gin, h, W[f"{o}.lstm0.ih.w"], rows * T, H, G, bias=W[f"{o}.lstm0.b"])
+        ginw = self._buf(tag + ".ginw", cap, G, dtype=gdt)
+        self._gather_rows(gin, ginw, i_gin1, W[f"{o}.lstm0.b"], n)
+        hw = self._buf(tag + ".hw", cap, 2 * H, dtype=self._adt(2 * H))
+        rec = dict(rows=n_seq, T=S, H=H, n_win=1, steps=S, stride=0, in_windowed=1, out_windowed=1, tc=tc)
+        self._lstm_rec(ginw[:n], W[f"{o}.lstm0.b"], whh0, hw[:n], **rec)
+        h1 = self._buf(tag + ".h1w", cap, 2 * H, dtype=hw.dtype)
+        self._gather_rows(hw, h1, i_h1, None, n)
+        g2dt = gdt if h1.dtype == torch.float16 else torch.float32
+        gin2 = self._buf(tag + ".gin2w", cap, G, dtype=g2dt)
+        self._gemm_flat(gin2, h1, W[f"{o}.lstm1.ih.w"], n, 2 * H, G, bias=W[f"{o}.lstm1.b"])
+        ginw = ginw if g2dt == gdt else self._buf(tag + ".ginw2", cap, G, dtype=g2dt)
+        self._gather_rows(gin2, ginw, i_gin2, W[f"{o}.lstm1.b"], n)
+        self._lstm_rec(ginw[:n], W[f"{o}.lstm1.b"], whh1, hw[:n], **rec)
+        h2 = self._buf(tag + ".h2", rows * T, 2 * H, dtype=self._adt(2 * H))
+        self._gather_rows(hw, h2, i_out, None, rows * T)
         self._gemm_flat(h, h2, W[o + ".lin.w"], rows * T, 2 * H, H, bias=W[o + ".lin.b"], residual=h, rnd=True)
         return h
 
@@ -669,8 +839,9 @@ class AeroEngine:
             st1 = self._stats.take(rows)
             h = self._buf(f"{tag}.h", B, Fq, T, hid, dtype=self._adt(hid))
             h_raw = self._raw(h, f"{tag}.h32")
-            self._gemm(h_raw, W[o + ".c1.w"], a1=y, B=B, F_out=Fq, T=T, N=hid, C1=Cc, kt=3, dil_t=dil, pad_t=dil,
-                       bias=W[o + ".c1.b"], stats=st1, stats_mode=2)
+            self._mask(y)
+            self._gemm_norm(h_raw, W[o + ".c1.w"], st1, scope=2, groups=1, a1=y, B=B, F_out=Fq, T=T, N=hid, C1=Cc, kt=3,
+                            dil_t=dil, pad_t=dil, bias=W[o + ".c1.b"])
             self._norm_act(h_raw, st1, W[o + ".n1.g"], W[o + ".n1.b"], h, B=B, F_in=Fq, T=T, C_=hid, groups=1, scope=2,
                            op=act, snake_a=W.get(o + ".a"), rnd=True)
             if g.lstm:
@@ -679,8 +850,8 @@ class AeroEngine:
                 self._local_attn(h, W, o, rows, T, hid, f"{tag}.attn")
             st2 = self._stats.take(rows)
             u = self._buf(f"{tag}.u", B, Fq, T, 2 * Cc, dtype=self._rdt(2 * Cc))
-            self._gemm(u, W[o + ".c2.w"], a1=h, B=B, F_out=Fq, T=T, N=2 * Cc, C1=hid, bias=W[o + ".c2.b"],
-                       stats=st2, stats_mode=2)
+            self._gemm_norm(u, W[o + ".c2.w"], st2, scope=2, groups=1, a1=h, B=B, F_out=Fq, T=T, N=2 * Cc, C1=hid,
+                            bias=W[o + ".c2.b"])
             self._norm_act(u, st2, W[o + ".n2.g"], W[o + ".n2.b"], y, B=B, F_in=Fq, T=T, C_=2 * Cc, groups=1, scope=2,
                            op=NA_GLU_SCALE_RES, scale=W[o + ".ls"], residual=y, rnd=True)
         return y
@@ -710,9 +881,8 @@ class AeroEngine:
         if g.norm:
             st = self._stats.take(B * kw["norm_groups"])
             y_raw = self._raw(y, tag + ".conv32")
-            self._gemm(y_raw, W[p + ".conv.w"], a1=x, B=B, F_out=Fo, F_in=Fi, T=T, N=Cc, C1=cin, kf=g.kernel,
-                       stride_f=g.stride, pad_f=g.pad, bias=W[p + ".conv.b"], stats=st, stats_mode=1,
-                       groups=kw["norm_groups"])
+            self._gemm_norm(y_raw, W[p + ".conv.w"], st, scope=1, groups=kw["norm_groups"], a1=x, B=B, F_out=Fo, F_in=Fi,
+                            T=T, N=Cc, C1=cin, kf=g.kernel, stride_f=g.stride, pad_f=g.pad, bias=W[p + ".conv.b"])
             self._norm_act(y_raw, st, W[p + ".norm1.g"], W[p + ".norm1.b"], y, B=B, F_in=Fo, T=T, C_=Cc,
                            groups=kw["norm_groups"], scope=1, op=NA_GELU, rnd=True)
         else:
@@ -724,8 +894,8 @@ class AeroEngine:
         if g.norm:
             st = self._stats.take(B * kw["norm_groups"])
             raw = self._buf(tag + ".rw", B, Fo, T, 2 * Cc, dtype=self._rdt(2 * Cc))
-            self._gemm(raw, W[p + ".rw.w"], a1=y, B=B, F_out=Fo, T=T, N=2 * Cc, C1=Cc, bias=W[p + ".rw.b"],
-                       stats=st, stats_mode=1, groups=kw["norm_groups"])
+            self._gemm_norm(raw, W[p + ".rw.w"], st, scope=1, groups=kw["norm_groups"], a1=y, B=B, F_out=Fo, T=T, N=2 * Cc,
+                            C1=Cc, bias=W[p + ".rw.b"])
             self._norm_act(raw, st, W[p + ".norm2.g"], W[p + ".norm2.b"], out, B=B, F_in=Fo, T=T, C_=2 * Cc,
                            groups=kw["norm_groups"], scope=1, op=NA_GLU, rnd=True)
         else:
@@ -740,6 +910,8 @@ class AeroEngine:
         tag = f"d{j}"
         Fq, Cc = g.f_out, g.ch
         c1 = 0 if x is None else Cc
+        self._mask(x)
+        self._mask(skip)
         # the last layer's GLU output feeds the exact-fp32 final transposed conv: kept in fp32 (-15 % end-to-end error for 75 MB)
         y = self._buf(tag + ".glu", B, Fq, T, 2 * Cc, dtype=torch.float32 if last else self._adt(2 * Cc))
         common = dict(a1=x, a2=skip, B=B, F_out=Fq, T=T, N=4 * Cc, C1=c1, C2=Cc, kf=3, kt=3, pad_f=1, pad_t=1,
@@ -747,7 +919,7 @@ class AeroEngine:
         if g.norm:
             st = self._stats.take(B * kw["norm_groups"])
             raw = self._buf(tag + ".rw", B, Fq, T, 4 * Cc, dtype=self._rdt(4 * Cc))
-            self._gemm(raw, W[p + ".rw.w"], stats=st, stats_mode=1, groups=kw["norm_groups"], **common)
+            self._gemm_norm(raw, W[p + ".rw.w"], st, scope=1, groups=kw["norm_groups"], **common)
             self._norm_act(raw, st, W[p + ".norm1.g"], W[p + ".norm1.b"], y, B=B, F_in=Fq, T=T, C_=4 * Cc,
                            groups=kw["norm_groups"], scope=1, op=NA_GLU, rnd=True)
         else:
@@ -760,9 +932,8 @@ class AeroEngine:
         if g.norm:
             st = self._stats.take(B * kw["norm_groups"])
             raw = self._buf(tag + ".ct", B, f_full, T, cout, dtype=self._rdt(cout))
-            self._gemm(raw, W[p + ".ct.w"], a1=y, B=B, F_out=f_full, F_in=Fq, T=T, N=cout, C1=2 * Cc, mode=TAPS_CONVT,
-                       kf=g.kernel, stride_f=g.stride, bias=W[p + ".ct.b"], stats=st, stats_mode=1,
-                       groups=kw["norm_groups"])
+            self._gemm_norm(raw, W[p + ".ct.w"], st, scope=1, groups=kw["norm_groups"], a1=y, B=B, F_out=f_full, F_in=Fq,
+                            T=T, N=cout, C1=2 * Cc, mode=TAPS_CONVT, kf=g.kernel, stride_f=g.stride, bias=W[p + ".ct.b"])
             self._norm_act(raw, st, W[p + ".norm2.g"], W[p + ".norm2.b"], z, B=B, F_in=f_full, F_out=f_keep,
                            f_off=g.pad, T=T, C_=cout, groups=kw["norm_groups"], scope=1,
                            op=cabi.NA_NONE if last else NA_GELU, rnd=not last)
@@ -817,6 +988,52 @@ class AeroEngine:
             graph.replay()
             return static_out.clone()
 
+    @torch.no_grad()
+    def forward_varlen(self, mix, lengths, return_spec=False, return_lr_spec=False):
+        """Ragged batch: clip b is mix[b, :, :lengths[b]] (samples past it are never read) and comes out as it does from
+        forward(mix[b:b+1, :, :lengths[b]]).  Returns the padded waveform [B, C_out, max out_len] and the list of per-clip
+        output lengths; with return_spec / return_lr_spec also the spectrograms over all T frames of the batch (each clip's
+        first frames are its own, the rest are zeros).  Runs eagerly: the launch sequence depends on the lengths; its workspaces
+        are released when it returns."""
+        self._require(mix)
+        self._check_mode()
+        g = self.geom
+        kw = g.kw
+        if mix.dim() != 3 or mix.shape[1] != kw["in_channels"]:
+            raise ValueError(f"expected input [B, {kw['in_channels']}, L], got {tuple(mix.shape)}")
+        lengths = [int(n) for n in lengths]
+        if len(lengths) != mix.shape[0]:
+            raise ValueError(f"{len(lengths)} lengths for a batch of {mix.shape[0]}")
+        if mix.shape[0] == 0:
+            out = self._forward(mix, return_spec, return_lr_spec)
+            return (out, []) if not return_spec else (out[0], [], *out[1:])
+        if any(n < 1 or n > mix.shape[2] for n in lengths):
+            raise ValueError(f"lengths must lie in [1, {mix.shape[2]}], got {lengths}")
+        hop = g.hop_in
+        short = [n for n in lengths if n + (-n) % hop <= g.nfft // 2]
+        if short:
+            # the single-clip forward rejects these in aero_stft_fwd (torch.stft does in the reference)
+            raise cabi.AeroLibraryError(f"aero_stft_varlen_fwd: reflect padding needs length ({short[0] + (-short[0]) % hop}) > "
+                                        f"n_fft/2 ({g.nfft // 2})")
+        with self._on_device():
+            frames = [1 + (n + (-n) % hop) // hop for n in lengths]
+            T = 1 + (mix.shape[2] + (-mix.shape[2]) % hop) // hop
+            out_lens = [min(int(n * g.scale), g.hop_out * (tb - 1)) for n, tb in zip(lengths, frames)]
+            keys = {(mix.shape[0] * lg.f_out, T) for lg in g.layers if lg.dconv and lg.lstm}
+            self._vl = _Ragged(frames, mix.device, lengths, out_lens, sorted(keys))
+            try:
+                out = self._forward(mix, return_spec, return_lr_spec, lengths=lengths)
+            finally:
+                self._vl = None
+                # the workspaces of a ragged batch are keyed on its exact longest clip, which rarely repeats in an evaluation
+                # loop: release them rather than keep up to max_shape_sets of them (tens of GB at 32 x 8 s)
+                self._bufsets.pop((tuple(mix.shape), self.precision, "varlen"), None)
+                self._bufs = {}
+        if not return_spec:
+            return out
+        (y, out_lens), *specs = out
+        return (y, out_lens, *specs)
+
     def _check_mode(self):
         if self.model.training:
             raise NotImplementedError(
@@ -824,7 +1041,7 @@ class AeroEngine:
                 "call model.eval().  Training kernels are SURVEY.md section 8f 'next'.")
 
     @torch.no_grad()
-    def _forward(self, mix, return_spec=False, return_lr_spec=False):
+    def _forward(self, mix, return_spec=False, return_lr_spec=False, lengths=None):
         self._require(mix)
         self._check_mode()
         g = self.geom
@@ -844,7 +1061,7 @@ class AeroEngine:
                 return y0, zc0
             return y0, zc0, torch.zeros(0, kw["in_channels"], Fq0, Tn, dtype=torch.complex64, device=mix.device)
         W = self._weights()
-        self._select_shape_set((tuple(mix.shape), self.precision))
+        self._select_shape_set((tuple(mix.shape), self.precision) + (() if lengths is None else ("varlen",)))
         B_ = mix.shape[0]
         need = B_ + sum((2 * B_ * kw["norm_groups"] if lg.norm else 0) * 2 +
                         (2 * abs(kw["dconv_depth"]) * B_ * lg.f_out if lg.dconv else 0) for lg in g.layers) + 64
@@ -868,16 +1085,24 @@ class AeroEngine:
         zrow = _pad4(T * C2)
         z = self._buf("z", B, Fq, zrow, zero=True)
         st_in = self._stats.take(B)
-        self.stft_into(x.view(B * Cin, Lp), z, st_in, n_fft=g.nfft, hop=g.hop_in, win=g.win_in, channels=Cin,
-                       bins_out=Fq, strides=(Fq * zrow, 2, zrow, C2))
         xn = self._buf("xn", B, Fq, zrow)
         affine = self._buf("affine", B, 2)
-        self._sample_norm(z, st_in, xn, affine, B, Fq * T * C2, extent=Fq * zrow)
+        if lengths is None:
+            self.stft_into(x.view(B * Cin, Lp), z, st_in, n_fft=g.nfft, hop=g.hop_in, win=g.win_in, channels=Cin,
+                           bins_out=Fq, strides=(Fq * zrow, 2, zrow, C2))
+            self._sample_norm(z, st_in, xn, affine, B, Fq * T * C2, extent=Fq * zrow)
+        else:
+            self.stft_varlen_into(x.view(B * Cin, Lp), self._vl.lengths_d, z, st_in, n_fft=g.nfft,
+                                  hop=g.hop_in, win=g.win_in, channels=Cin, bins_out=Fq, strides=(Fq * zrow, 2, zrow, C2))
+            self._sample_norm_varlen(z, st_in, xn, affine, B, Fq * C2, Fq * zrow)
         xr = None
         l0 = g.layers[0]
         if self.precision >= 1 and l0.ftb and self.fuse_pre_ftb:
             xr = self._buf("xnr", B, Fq, zrow)        # TF32-rounded copy: the tensor-core operand of the frequency mix
-            self._sample_norm(z, st_in, xr, affine, B, Fq * T * C2, extent=Fq * zrow, rnd=True)
+            if lengths is None:
+                self._sample_norm(z, st_in, xr, affine, B, Fq * T * C2, extent=Fq * zrow, rnd=True)
+            else:
+                self._sample_norm_varlen(z, st_in, xr, affine, B, Fq * C2, Fq * zrow, rnd=True)
         h = xn
         saved = []
         for lg in g.layers:
@@ -890,13 +1115,24 @@ class AeroEngine:
         Cout = kw["out_channels"]
         assert h.shape == (B, Fq, T, 2 * Cout), (h.shape, (B, Fq, T, 2 * Cout))
 
-        out_len = min(int(length * g.scale), g.hop_out * (T - 1))
-        y = torch.empty(B * Cout, out_len, dtype=torch.float32, device=mix.device)
-        self.istft_into(h, y, n_fft=g.nfft, hop=g.hop_out, win=g.win_out, channels=Cout, frames=T, bins_in=Fq,
-                        strides=(Fq * T * 2 * Cout, 2, T * 2 * Cout, 2 * Cout))
-        y = y.view(B, Cout, out_len)
+        strides = (Fq * T * 2 * Cout, 2, T * 2 * Cout, 2 * Cout)
+        if lengths is None:
+            out_len = min(int(length * g.scale), g.hop_out * (T - 1))
+            y = torch.empty(B * Cout, out_len, dtype=torch.float32, device=mix.device)
+            self.istft_into(h, y, n_fft=g.nfft, hop=g.hop_out, win=g.win_out, channels=Cout, frames=T, bins_in=Fq,
+                            strides=strides)
+            y = y.view(B, Cout, out_len)
+        else:
+            out_lens = [min(int(n * g.scale), g.hop_out * (tb - 1)) for n, tb in zip(lengths, self._vl.frames)]
+            out_len = max(out_lens)
+            y = torch.empty(B * Cout, out_len, dtype=torch.float32, device=mix.device)
+            self.istft_varlen_into(h, y, self._vl.frames_d, self._vl.out_lens_d, n_fft=g.nfft,
+                                   hop=g.hop_out, win=g.win_out, channels=Cout, frames_max=T, bins_in=Fq, strides=strides)
+            y = (y.view(B, Cout, out_len), out_lens)
         if not return_spec:
             return y
+        if lengths is not None:
+            self._frame_mask(h)          # padded frames of the returned spectrogram are zeros, not workspace contents
         zc = torch.view_as_complex(h.clone().view(B, Fq, T, Cout, 2)).permute(0, 3, 1, 2)
         if not return_lr_spec:
             return y, zc

@@ -6,6 +6,9 @@
   statistics, ``aero.py:462-464``) and concatenate.  The reference runs the chunks one by one at batch 1 with a
   host round trip per chunk; here equal-length chunks go through the kernels as one batch and stay on the device.
   Results are identical to the serial loop because samples of a batch never interact.
+* ``enhance_batch(model, signals)``          -- many clips of different lengths (reference ``test.py`` / ``evaluate.py``,
+  many-file ``predict.py``): sorted by length and run in ragged batches (``AeroEngine.forward_varlen``), each clip with
+  the result it gets on its own.
 """
 from __future__ import annotations
 
@@ -48,3 +51,46 @@ def enhance_long(model, lr_sig, sr, segment_sec=SEGMENT_DURATION_SEC, max_batch=
         tail = lr_sig[:, n_full * seg:]
         outs.append(model(tail.unsqueeze(0))[0])
     return torch.cat(outs, dim=-1)
+
+
+@torch.no_grad()
+def enhance_batch(model, signals, max_batch=32, return_spec=False, return_lr_spec=False):
+    """signals: list of [C, L_i] tensors on the model's (CUDA) device at ``model.lr_sr``.  Returns a list, in input order,
+    of what ``model(signals[i][None])`` returns with the batch axis dropped: the waveform [C_out, out_len(L_i)], and with
+    ``return_spec`` / ``return_lr_spec`` the spectrograms cropped to the clip's own frames.  Clips are sorted by length and
+    run in ragged batches of at most ``max_batch``, so that each batch carries as little padding as possible."""
+    from .model import Aero
+    if not isinstance(model, Aero):
+        raise NotImplementedError(f"enhance_batch runs the AERO generator only, got {type(model).__name__}")
+    eng = model._engine()
+    if model.training:
+        eng._check_mode()
+    if max_batch < 1:
+        raise ValueError(f"max_batch must be >= 1, got {max_batch}")
+    signals = list(signals)
+    if not signals:
+        return []
+    cin = model.geom.kw["in_channels"]
+    for i, s in enumerate(signals):
+        eng._require(s)
+        if s.dim() != 2 or s.shape[0] != cin:
+            raise ValueError(f"signal {i}: expected [{cin}, L], got {tuple(s.shape)}")
+    order = sorted(range(len(signals)), key=lambda i: signals[i].shape[-1])
+    results = [None] * len(signals)
+    for k in range(0, len(order), max_batch):
+        idx = order[k:k + max_batch]
+        lens = [signals[i].shape[-1] for i in idx]
+        mix = signals[idx[0]].new_zeros(len(idx), cin, max(lens))
+        for j, i in enumerate(idx):
+            mix[j, :, :lens[j]] = signals[i]
+        out = eng.forward_varlen(mix, lens, return_spec=return_spec, return_lr_spec=return_lr_spec)
+        y, out_lens = out[0], out[1]
+        frames = [model.geom.frames(n) for n in lens]
+        for j, i in enumerate(idx):
+            r = y[j, :, :out_lens[j]].clone()
+            if return_spec:
+                specs = tuple(sp[j, ..., :frames[j]].clone() for sp in out[2:])
+                results[i] = (r, *specs)
+            else:
+                results[i] = r
+    return results

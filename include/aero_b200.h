@@ -537,6 +537,50 @@ int aero_gan_loss_fwd(const aero_gan_term* terms, int32_t n_terms, double* out, 
  * disjoint element ranges. */
 int aero_gan_loss_bwd(const aero_gan_term* terms, int32_t n_terms, aero_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Ragged batches: clips of different lengths in one forward, each with the result it gets on its own.
+ * Clip b occupies the first frames[b] frames of the usual [B][F][T][C] tensors (T = the batch's longest clip); the rest are
+ * padding.  Padded frames are left out of every reduction and sequence op, and hold exact zeros in every tensor a
+ * time-coupled convolution reads.  Length tables (`lengths`, `frames`, `out_lens`) are int32 DEVICE arrays with one entry per
+ * clip.
+ *
+ * aero_stft_varlen_fwd: aero_stft_fwd for signals of lengths[b] valid samples in rows of p->length (a multiple of hop;
+ *   p->frames = 1 + length/hop).  Each signal is zero padded to a multiple of hop and reflected at that padded end
+ *   (reference aero.py:409-420, spec.py:9-22, on the clip alone); frames at or past its own 1 + padded/hop are written as
+ *   zeros, and stats[b] accumulates {sum, sumsq} over its valid frames only.  p->flags must be 0.
+ *   Preconditions (the caller's; they cannot be checked without reading the device table): 1 <= lengths[b] <= p->length and
+ *   lengths[b] padded to a multiple of hop > n_fft/2 (reflect padding, as for aero_stft_fwd).  Out of contract, the kernel
+ *   clamps lengths[b] to p->length and reads no sample outside the signal's row (such frames are garbage, not a fault).
+ */
+int aero_stft_varlen_fwd(const float* x, const float* window, float* z, double* stats, const int32_t* lengths,
+                         const aero_stft_params* p, aero_stream_t stream);
+/* aero_istft_varlen_fwd: aero_istft_fwd where signal b uses frames[b] frames and writes out_lens[b] samples of its row of
+ *   p->out_len (the rest of the row is zeroed).  p->flags must be 0. */
+int aero_istft_varlen_fwd(const float* z, const float* window, float* y, const int32_t* frames, const int32_t* out_lens,
+                          const aero_istft_params* p, aero_stream_t stream);
+/* aero_sample_norm_varlen_fwd: aero_sample_norm_fwd with each clip's own count, per_frame * frames[b] values; `extent`
+ *   floats per sample are transformed. */
+int aero_sample_norm_varlen_fwd(const float* x, const double* stats, float* y, float* samp_affine, const int32_t* frames,
+                                int32_t B, int64_t per_frame, int64_t extent, int32_t round_tf32, aero_stream_t stream);
+/* aero_masked_stats_fwd: GroupNorm statistics of a stored tensor x [B][F][T][C] (fp32, or FP16 with AERO_TG_A_F16) over
+ *   the valid frames t < frames[b] only, added into the slots aero_norm_act_fwd reads (scope 1: [B][groups]; scope 2:
+ *   [B*F]), scaled by T / frames[b] so that norm_act's count over T frames gives the clip's own mean and variance. */
+int aero_masked_stats_fwd(const void* x, double* stats, const int32_t* frames, int32_t B, int32_t F, int32_t T, int32_t C,
+                          int32_t groups, int32_t scope, int32_t flags, aero_stream_t stream);
+/* aero_frame_mask_fwd: x [B][F][T][C] (fp32, or FP16 with AERO_TG_OUT_F16): frames t >= frames[b] are set to zero. */
+int aero_frame_mask_fwd(void* x, const int32_t* frames, int32_t B, int32_t F, int32_t T, int32_t C, int32_t flags,
+                        aero_stream_t stream);
+/* aero_gather_rows_fwd: dst[i][c] = src[idx[i*parts + c/(width/parts)]][c] for rows of `width` elements (fp32, or FP16 with
+ *   AERO_TG_A_F16); a negative index takes fill[c] (fp32; zero when fill is NULL).  The ragged BiLSTM uses it to lay each
+ *   clip's sequences (its own step count, windows of reference modules.py:32-65 past 200 frames, bias-only input past its
+ *   end, the reverse direction starting at its own last step) onto the windowed layout of aero_lstm_rec_fwd and back. */
+int aero_gather_rows_fwd(const void* src, void* dst, const int32_t* idx, const float* fill, int64_t n_rows, int32_t width,
+                         int32_t parts, int32_t flags, aero_stream_t stream);
+/* aero_local_attn_varlen_fwd: aero_local_attn_fwd where row r belongs to clip r / rows_per_clip and only its first
+ *   frames[clip] frames take part (keys, queries, decay, softmax); outputs of the padded frames are not written. */
+int aero_local_attn_varlen_fwd(const float* qkvd, void* out, const int32_t* frames, int32_t rows_per_clip,
+                               const aero_attn_params* p, aero_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
