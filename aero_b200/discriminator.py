@@ -83,7 +83,6 @@ class _DiscEngine(TrainEngine):
         self.model = module
         self.geom = None
         self.lib = cabi.load()
-        self._windows = {}
         self.precision = int(getattr(module, "train_precision", 0))
         self._reset()
 

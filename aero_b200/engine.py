@@ -15,7 +15,7 @@ import math
 
 import torch
 
-from . import cabi
+from . import cabi, spec
 from .cabi import (ACT_GELU, ACT_NONE, ACT_RELU, NA_GELU, NA_GLU, NA_GLU_SCALE_RES, NA_RELU, NA_SNAKE, TAPS_CONV,
                    TAPS_CONVT)
 
@@ -205,7 +205,6 @@ class AeroEngine:
         self._bufs = {}
         self.max_shape_sets = 4
         self._plist = None
-        self._windows = {}
         self._stats = None
         # 2 (default): FP16-stored activations / f16 wgmma operands, fp32 accumulate, fp32 GroupNorm inputs and
         #    gate pre-activations -- TF32's 10-bit mantissa at half the HBM bytes and twice the tensor-core rate;
@@ -312,15 +311,6 @@ class AeroEngine:
         """Buffer for a pre-normalisation GEMM output whose normalised form is `like`: `like` itself (norm_act runs in
         place) when the storage types agree, else a separate fp32 buffer."""
         return like if like.dtype == self._rdt(like.shape[-1]) else self._buf(name, *like.shape)
-
-    def _window(self, win):
-        key = (win, self._device())
-        w = self._windows.get(key)
-        if w is None:
-            # computed on the host in fp32 exactly as reference spec.py:15 does, then moved
-            w = torch.hann_window(win).to(self._device())
-            self._windows[key] = w
-        return w
 
     def _weights(self):
         key = self._weights_version()
@@ -626,32 +616,22 @@ class AeroEngine:
                                                  C.byref(p), self._stream()), self.lib)
         return out
 
-    def stft_into(self, x, z, stats, *, n_fft, hop, win, channels, bins_out, strides):
-        n_sig, length = x.shape[0], x.shape[1]
-        frames = 1 + length // hop
-        p = cabi.StftParams(n_fft, hop, win, n_sig, channels, length, frames, bins_out, *strides)
-        rc = self.lib.aero_stft_fwd(_ptr(x), _ptr(self._window(win)), _ptr(z), _ptr(stats), C.byref(p), self._stream())
-        cabi.check(rc, self.lib)
+    # The STFT launches (aero_b200.spec) on the engine's stream.  These four methods and _window are the seam the CPU
+    # emulation (tests/cpu_emu.py, tests/test_ragged_host.py) and tools/traffic_model.py replace.
+    def _window(self, win):
+        return spec.window(win, self._device())
 
-    def stft_varlen_into(self, x, lengths, z, stats, *, n_fft, hop, win, channels, bins_out, strides):
-        n_sig, length = x.shape[0], x.shape[1]
-        p = cabi.StftParams(n_fft, hop, win, n_sig, channels, length, 1 + length // hop, bins_out, *strides)
-        rc = self.lib.aero_stft_varlen_fwd(_ptr(x), _ptr(self._window(win)), _ptr(z), _ptr(stats), _ptr(lengths), C.byref(p),
-                                           self._stream())
-        cabi.check(rc, self.lib)
+    def stft_into(self, x, z, stats, **kw):
+        spec.stft_into(x, z, stats, stream=self._stream(), **kw)
 
-    def istft_varlen_into(self, z, y, frames, out_lens, *, n_fft, hop, win, channels, frames_max, bins_in, strides):
-        n_sig, out_len = y.shape
-        p = cabi.IstftParams(n_fft, hop, win, n_sig, channels, frames_max, bins_in, out_len, *strides)
-        rc = self.lib.aero_istft_varlen_fwd(_ptr(z), _ptr(self._window(win)), _ptr(y), _ptr(frames), _ptr(out_lens), C.byref(p),
-                                            self._stream())
-        cabi.check(rc, self.lib)
+    def stft_varlen_into(self, x, lengths, z, stats, **kw):
+        spec.stft_into(x, z, stats, lengths=lengths, stream=self._stream(), **kw)
 
-    def istft_into(self, z, y, *, n_fft, hop, win, channels, frames, bins_in, strides):
-        n_sig, out_len = y.shape
-        p = cabi.IstftParams(n_fft, hop, win, n_sig, channels, frames, bins_in, out_len, *strides)
-        rc = self.lib.aero_istft_fwd(_ptr(z), _ptr(self._window(win)), _ptr(y), C.byref(p), self._stream())
-        cabi.check(rc, self.lib)
+    def istft_into(self, z, y, **kw):
+        spec.istft_into(z, y, stream=self._stream(), **kw)
+
+    def istft_varlen_into(self, z, y, frames, out_lens, *, frames_max, **kw):
+        spec.istft_into(z, y, frames=frames_max, clip_frames=frames, out_lens=out_lens, stream=self._stream(), **kw)
 
     # ------------------------------------------------------------------ public pieces
     @torch.no_grad()

@@ -18,7 +18,7 @@ import ctypes as C
 import torch
 
 from . import cabi
-from .spec import spectro, _window
+from .spec import spectro, stft_adjoint_into
 
 
 def _spectra(x, y, resolutions):
@@ -68,16 +68,7 @@ class _MRSTFTFn(torch.autograd.Function):
                 gz = torch.empty_like(zx)
                 cabi.check(lib.aero_stft_loss_bwd(C.c_void_p(zx.data_ptr()), C.c_void_p(zy.data_ptr()), C.c_void_p(ctx.sums[i].data_ptr()),
                                                   C.c_void_p(gz.data_ptr()), B, bins, frames, n_fft, k_sc, k_mag, stream), lib)
-                span = hop * (frames - 1) + n_fft                    # padded positions covered by a frame (<= L + n_fft)
-                gp = torch.empty(B, span, device=dev)
-                p = cabi.IstftParams(n_fft, hop, win, B, 1, frames, bins, span, bins * frames * 2, 0, frames * 2, 2, cabi.ISTFT_RAW, 0)
-                cabi.check(lib.aero_istft_fwd(C.c_void_p(gz.data_ptr()), C.c_void_p(_window(win, dev).data_ptr()), C.c_void_p(gp.data_ptr()),
-                                              C.byref(p), stream), lib)
-                gp = torch.nn.functional.pad(gp, (0, L + n_fft - span))
-                h = n_fft // 2
-                dx += gp[:, h:h + L]
-                dx[:, 1:h + 1] += gp[:, :h].flip(1)                  # left reflection: padded pos p < h came from x[h - p]
-                dx[:, L - 1 - h:L - 1] += gp[:, h + L:].flip(1)      # right reflection: padded pos h + L + j came from x[L - 2 - j]
+                stft_adjoint_into(gz, dx, n_fft=n_fft, hop=hop, win=win, stream=stream)
         return dx.to(ctx.dtype), None, None, None, None
 
 

@@ -59,49 +59,24 @@ def _(z, hop, win, length):
 
 def _stft_adjoint(g, n_fft, hop, win, length):
     """d loss / d x [..., length] from g = d loss / d z [..., bins, frames, 2] of z = stft(x) (normalised, centred, reflect)."""
-    import ctypes as C
-    from . import cabi
-    lib = cabi.load()
     lead = g.shape[:-3]
     bins, frames = g.shape[-3], g.shape[-2]
     gz = g.reshape(-1, bins, frames, 2).float().clone()
     gz[:, 1:bins - 1] *= 0.5                                   # interior bins count twice in the C2R transform
-    B = gz.shape[0]
-    span = hop * (frames - 1) + n_fft
-    gp = torch.empty(B, span, device=g.device)
+    dx = torch.zeros(gz.shape[0], length, device=g.device)
     with torch.cuda.device(g.device):
-        p = cabi.IstftParams(n_fft, hop, win, B, 1, frames, bins, span, bins * frames * 2, 0, frames * 2, 2, cabi.ISTFT_RAW, 0)
-        cabi.check(lib.aero_istft_fwd(C.c_void_p(gz.data_ptr()), C.c_void_p(spec._window(win, g.device).data_ptr()), C.c_void_p(gp.data_ptr()),
-                                      C.byref(p), C.c_void_p(torch.cuda.current_stream().cuda_stream)), lib)
-    gp = torch.nn.functional.pad(gp, (0, length + n_fft - span))
-    h = n_fft // 2
-    dx = gp[:, h:h + length].clone()
-    dx[:, 1:h + 1] += gp[:, :h].flip(1)
-    dx[:, length - 1 - h:length - 1] += gp[:, h + length:].flip(1)
+        spec.stft_adjoint_into(gz, dx, n_fft=n_fft, hop=hop, win=win, stream=spec.current_stream())
     return dx.view(*lead, length)
 
 
 def _istft_adjoint(gy, hop, win, bins, frames):
     """d loss / d z [..., bins, frames, 2] from gy = d loss / d y [..., length] of y = istft(z)."""
-    import ctypes as C
-    from . import cabi
-    lib = cabi.load()
-    n_fft = 2 * (bins - 1)
     lead, length = gy.shape[:-1], gy.shape[-1]
-    full = hop * (frames - 1)
-    w = torch.zeros(n_fft, device=gy.device)
-    wl = (n_fft - win) // 2
-    w[wl:wl + win] = spec._window(win, gy.device)
-    env = torch.nn.functional.fold((w * w).view(1, n_fft, 1).expand(1, n_fft, frames), (1, full + n_fft), (1, n_fft), stride=(1, hop)).reshape(-1)
-    u = torch.zeros(gy.numel() // length, full, device=gy.device)
-    u[:, :min(length, full)] = gy.reshape(-1, length)[:, :full].float()
-    u.div_(env[n_fft // 2:n_fft // 2 + full])
-    gz = torch.empty(u.shape[0], bins, frames, 2, device=gy.device)
+    gy = gy.reshape(-1, length)
+    gz = torch.empty(gy.shape[0], bins, frames, 2, device=gy.device)
     with torch.cuda.device(gy.device):
-        p = cabi.StftParams(n_fft, hop, win, u.shape[0], 1, full, frames, bins, bins * frames * 2, 0, frames * 2, 2,
-                            cabi.STFT_ZERO_PAD | cabi.STFT_ADJ_SCALE, 0)
-        cabi.check(lib.aero_stft_fwd(C.c_void_p(u.data_ptr()), C.c_void_p(spec._window(win, gy.device).data_ptr()), C.c_void_p(gz.data_ptr()), None,
-                                     C.byref(p), C.c_void_p(torch.cuda.current_stream().cuda_stream)), lib)
+        spec.istft_adjoint_into(gy, gz, n_fft=2 * (bins - 1), hop=hop, win=win, channels=1, frames=frames, bins=bins,
+                                strides=(bins * frames * 2, 0, frames * 2, 2), stream=spec.current_stream())
     return gz.view(*lead, bins, frames, 2)
 
 

@@ -462,7 +462,6 @@ class SeanetTrainEngine(TrainEngine):
         self.model = model
         self.geom = None
         self.lib = cabi.load()
-        self._windows = {}
         self.precision = int(getattr(model, "train_precision", 0))
         self._reset()
 

@@ -21,7 +21,7 @@ import math
 
 import torch
 
-from . import cabi
+from . import cabi, spec
 from .cabi import ACT_NONE, NA_GELU, NA_GLU, NA_GLU_SCALE_RES, NA_NO_NORM, NA_NONE, NA_RELU, NA_SNAKE, TAPS_CONV, TAPS_CONVT
 from .engine import _ATTN_HEADS, _ATTN_NDECAY, _LSTM_MAX_STEPS, dconv_norm_act_op, pack_taps, tf32_round
 
@@ -52,7 +52,6 @@ class TrainEngine:
         self.model = model
         self.geom = model.geom
         self.lib = cabi.load()
-        self._windows = {}
         # Arithmetic of the convolutions' forward, data-gradient and weight-gradient GEMMs (normalisation, LSTM recurrence, attention and
         # all reductions are fp32 / fp64 in every mode):
         #   0  exact-fp32 SIMT tap-GEMMs (the original gradient-parity mode);
@@ -143,12 +142,6 @@ class TrainEngine:
                 t = torch.zeros_like(self.params[name], dtype=torch.float32, memory_format=torch.contiguous_format)
             self.pg[name] = t
         return t
-
-    def _window(self, win):
-        w = self._windows.get((win, self._device()))
-        if w is None:
-            w = self._windows[(win, self._device())] = torch.hann_window(win).to(self._device())
-        return w
 
     # ------------------------------------------------------------------ kernel wrappers
     def _tg(self, *, B, F_out, T, N, C1, C2=0, F_in=None, a1_s=None, a2_s=None, o_s=None, mode=TAPS_CONV, kf=1, kt=1, stride_f=1,
@@ -738,8 +731,8 @@ class TrainEngine:
         # STFT straight into channels-last [B, F, T, 2*Cin] (aero.py:409-434) + per-sample standardisation (aero.py:462-464)
         z = self._new(B, Fq, T, C2)
         st_in = self._new(B, 2, zero=True, dtype=torch.float64)
-        sp = cabi.StftParams(g.nfft, g.hop_in, g.win_in, B * Cin, Cin, Lp, T, Fq, Fq * T * C2, 2, T * C2, C2)
-        self._check(lib.aero_stft_fwd(_ptr(x.view(B * Cin, Lp)), _ptr(self._window(g.win_in)), _ptr(z), _ptr(st_in), C.byref(sp), self._stream()))
+        spec.stft_into(x.view(B * Cin, Lp), z, st_in, n_fft=g.nfft, hop=g.hop_in, win=g.win_in, channels=Cin, bins_out=Fq,
+                       strides=(Fq * T * C2, 2, T * C2, C2), stream=self._stream())
         xn = self._new(B, Fq, T, C2)
         affine = self._new(B, 2)
         self._check(lib.aero_sample_norm_fwd(_ptr(z), _ptr(st_in), _ptr(xn), _ptr(affine), B, Fq * T * C2, Fq * T * C2, 0, self._stream()))
@@ -757,45 +750,21 @@ class TrainEngine:
         Cout = kw["out_channels"]
         out_len = min(int(length * g.scale), g.hop_out * (T - 1))
         y = self._new(B * Cout, out_len)
-        ip = cabi.IstftParams(g.nfft, g.hop_out, g.win_out, B * Cout, Cout, T, Fq, out_len, Fq * T * 2 * Cout, 2, T * 2 * Cout, 2 * Cout)
-        self._check(lib.aero_istft_fwd(_ptr(h), _ptr(self._window(g.win_out)), _ptr(y), C.byref(ip), self._stream()))
+        spec.istft_into(h, y, n_fft=g.nfft, hop=g.hop_out, win=g.win_out, channels=Cout, frames=T, bins_in=Fq,
+                        strides=(Fq * T * 2 * Cout, 2, T * 2 * Cout, 2 * Cout), stream=self._stream())
         self._final = (h, B, Cout, T, Fq, out_len)
         self.keep.append((z, xn, affine, x))
         return y.view(B, Cout, out_len), h.view(B, Fq, T, 2 * Cout)
 
     # ------------------------------------------------------------------ backward
-    def _envelope(self, T):
-        """sum_t w^2[pos - t*hop] of the synthesis window over the padded axis (what torch.istft divides by)."""
-        g = self.geom
-        key = (T, self._device())
-        e = self._env_cache.get(key) if hasattr(self, "_env_cache") else None
-        if e is None:
-            if not hasattr(self, "_env_cache"):
-                self._env_cache = {}
-            N, hop = g.nfft, g.hop_out
-            w = torch.zeros(N, device=self._device())
-            wl = (N - g.win_out) // 2
-            w[wl:wl + g.win_out] = self._window(g.win_out)
-            w2 = (w * w).view(1, N, 1).expand(1, N, T)
-            e = torch.nn.functional.fold(w2, (1, hop * (T - 1) + N), (1, N), stride=(1, hop)).reshape(-1)
-            self._env_cache[key] = e
-        return e
-
     @torch.no_grad()
     def istft_adjoint(self, d_wave, B, Cout, T, Fq, out_len):
-        """Gradient of the output spectrogram [B, Fq, T, 2 C_out] from the gradient of the waveform: the adjoint of
-        aero_istft_fwd = zero-extend, divide by the window envelope, then the STFT kernel with zero padding and the C2R
-        adjoint scaling (include/aero_b200.h, AERO_STFT_ZERO_PAD | AERO_STFT_ADJ_SCALE)."""
+        """Gradient of the output spectrogram [B, Fq, T, 2 C_out] from the gradient of the waveform (the adjoint of
+        aero_istft_fwd, aero_b200.spec.istft_adjoint_into)."""
         g = self.geom
-        N, hop = g.nfft, g.hop_out
-        full = hop * (T - 1)
-        u = torch.zeros(B * Cout, full, device=d_wave.device)
-        u[:, :out_len] = d_wave.reshape(B * Cout, out_len).float()
-        u.div_(self._envelope(T)[N // 2:N // 2 + full])
         dz = self._new(B, Fq, T, 2 * Cout)
-        sp = cabi.StftParams(N, hop, g.win_out, B * Cout, Cout, full, T, Fq, Fq * T * 2 * Cout, 2, T * 2 * Cout, 2 * Cout,
-                             cabi.STFT_ZERO_PAD | cabi.STFT_ADJ_SCALE, 0)
-        self._check(self.lib.aero_stft_fwd(_ptr(u), _ptr(self._window(g.win_out)), _ptr(dz), None, C.byref(sp), self._stream()))
+        spec.istft_adjoint_into(d_wave.reshape(B * Cout, out_len), dz, n_fft=g.nfft, hop=g.hop_out, win=g.win_out, channels=Cout,
+                                frames=T, bins=Fq, strides=(Fq * T * 2 * Cout, 2, T * 2 * Cout, 2 * Cout), stream=self._stream())
         return dz
 
     @torch.no_grad()
