@@ -23,7 +23,7 @@ import torch
 
 from . import cabi, spec
 from .cabi import ACT_NONE, NA_GELU, NA_GLU, NA_GLU_SCALE_RES, NA_NO_NORM, NA_NONE, NA_RELU, NA_SNAKE, TAPS_CONV, TAPS_CONVT
-from .engine import _ATTN_HEADS, _ATTN_NDECAY, _LSTM_MAX_STEPS, dconv_norm_act_op, pack_taps, tf32_round
+from .engine import _ATTN_HEADS, _ATTN_NDECAY, _LSTM_MAX_STEPS, center_groups, dconv_norm_act_op, pack_taps, tf32_round
 
 _FTB_R, _FTB_RP = 5, 8          # FTB squeeze channels (modules.py:286) and their padded count (kernels work on channel quads)
 
@@ -271,6 +271,10 @@ class TrainEngine:
             bias, b_back = b_override
         else:
             bias, b_back = (P[bname] if bname else None), None
+            if stats is not None and bias is not None:
+                # the output feeds a GroupNorm: store it without the groups' common bias offset (engine.center_groups).  The
+                # shift is piecewise constant in the bias, so the column sums below stay the bias gradient as they are.
+                bias = center_groups(bias, groups if stats_mode == 1 else 1)
         if cv.kind == "conv":
             w4 = w.reshape(N, K, cv.kf, cv.kt)
             wp = pack_taps(w4.reshape(N, K, cv.kf * cv.kt))

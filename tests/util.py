@@ -4,6 +4,8 @@ import sys
 
 import numpy as np
 import torch
+import torch.nn.functional as F
+from torch.overrides import TorchFunctionMode
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
@@ -107,3 +109,52 @@ def disc_recipe_state(state, seed=SEED):
         elif k.endswith("bias"):
             out[k] = 0.05 * r
     return {k: out[k].to(state[k].dtype) for k in state}
+
+
+class _PreNormTrace(TorchFunctionMode):
+    """Records (weight key, bias key, groups) for every conv call whose output goes straight into group_norm."""
+    CONVS = {F.conv1d, F.conv2d, F.conv_transpose2d, torch.conv1d, torch.conv2d, torch.conv_transpose2d}
+
+    def __init__(self, sd):
+        super().__init__()
+        self.key = {id(v): k for k, v in sd.items()}
+        self.made = {}
+        self.found = []
+
+    def __torch_function__(self, func, types, args=(), kwargs=None):
+        kwargs = kwargs or {}
+        out = func(*args, **kwargs)
+        if func in self.CONVS:
+            bias = args[2] if len(args) > 2 else kwargs.get("bias")
+            self.made[id(out)] = (out, self.key.get(id(args[1])), self.key.get(id(bias)))
+        elif func is F.group_norm:
+            src = self.made.get(id(args[0]))
+            groups = args[1] if len(args) > 1 else kwargs["num_groups"]
+            if src is not None and src[0] is args[0]:
+                self.found.append((src[1], src[2], groups))
+        return out
+
+
+def pre_norm_convs(model):
+    """[(weight key, bias key, groups)] of the convolutions that feed a GroupNorm, in forward order."""
+    from oracle import aero_oracle as O
+    sd = {k: v.clone() for k, v in model.state_dict().items()}
+    tr = _PreNormTrace(sd)
+    with torch.no_grad(), tr:
+        O.aero_forward(sd, model.geom, white_noise((1, model.in_channels, 2000), seed=3))
+    assert tr.found and all(w and b for w, b, _ in tr.found), tr.found
+    return tr.found
+
+
+def shifted(sd, layers, c):
+    """`sd` with a constant added to the bias of each GroupNorm group of every pre-normalisation conv (`layers` from
+    pre_norm_convs): the same function for any c, as GroupNorm subtracts each group's mean.  The constants differ between the
+    groups of a conv and between convs, c_i = c (-1)^i (1 + 0.37 (i mod 4)) with i = group index + conv index, so that a
+    per-group shift undone with the wrong grouping changes the result, and most of them are not multiples of 1/8, so that
+    part of each offset stays in the stored pre-normalisation values."""
+    out = {k: v.clone() for k, v in sd.items()}
+    for j, (_, b, groups) in enumerate(layers):
+        n = out[b].numel()
+        i = torch.arange(n) // (n // groups) + j
+        out[b] += (c * (-1.0) ** i * (1 + 0.37 * (i % 4))).to(out[b].dtype)
+    return out
