@@ -100,6 +100,7 @@ SYMBOLS = {
     "aero_lstm_tc_shape": (C.c_int, [i32, i32, i32, C.POINTER(i32)]),
     "aero_local_attn_fwd": (C.c_int, [vp, vp, C.POINTER(AttnParams), vp]),
     "aero_lsd_fwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, vp]),
+    "aero_lsd_varlen_fwd": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, vp, vp]),
     "aero_stft_loss_fwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "aero_stft_loss_bwd": (C.c_int, [vp, vp, vp, vp, i32, i32, i32, i32, f32, f32, vp]),
     # training (SURVEY.md section 8f rank 1)

@@ -11,38 +11,11 @@
 // A CTA owns a run of consecutive frames of one signal so that, for every frequency bin, the
 // frames it writes (reads) are contiguous in memory: >=128 B segments for the model's layouts.
 #include "common.cuh"
+#include "fft.cuh"
 
 namespace aero {
 
 constexpr int kThreads = 256;
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-    return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
-}
-
-// In-place radix-2 DIT over `nfr` frames of M = 2^LOGM complex points, input in bit-reversed
-// order, twiddles tw[j] = exp(-+2 pi i j / (2M)) (table over N = 2M), sign chosen by table.
-template <int LOGM>
-__device__ __forceinline__ void fft_inplace(float2* work, const float2* twN, int nfr) {
-    constexpr int M = 1 << LOGM;
-    const int total = nfr * (M / 2);
-#pragma unroll 1
-    for (int s = 0; s < LOGM; ++s) {
-        const int half = 1 << s;
-        const int tw_step = M >> s;          // N / (2*half) = 2M / (2*half)
-        for (int i = threadIdx.x; i < total; i += kThreads) {
-            const int fr = i / (M / 2), j = i - fr * (M / 2);
-            const int pos = j & (half - 1);
-            const int i0 = ((j >> s) << (s + 1)) + pos;
-            float2* w = work + fr * M;
-            const float2 a = w[i0];
-            const float2 b = cmul(w[i0 + half], twN[pos * tw_step]);
-            w[i0] = make_float2(a.x + b.x, a.y + b.y);
-            w[i0 + half] = make_float2(a.x - b.x, a.y - b.y);
-        }
-        __syncthreads();
-    }
-}
 
 template <int LOGN>
 struct StftCfg {
@@ -116,7 +89,7 @@ __device__ __forceinline__ void stft_block(const float* __restrict__ x, const fl
         work[fr * M + r] = make_float2(s[0] * wpad[2 * n], s[1] * wpad[2 * n + 1]);
     }
     __syncthreads();
-    fft_inplace<LOGM>(work, twN, nfr);
+    fft_inplace<LOGM, kThreads>(work, twN, nfr);
 
     // split post-pass: X[k] = Xe[k] + w^k Xo[k], X[M-k] = conj(Xe[k] - w^k Xo[k])
     const float scale = rsqrtf((float)N);
@@ -278,7 +251,7 @@ __device__ __forceinline__ void istft_block(const float* __restrict__ z, const f
         work[fr * M + r] = make_float2(xe.x - xo.y, xe.y + xo.x);      // xe + i*xo
     }
     __syncthreads();
-    fft_inplace<LOGM>(work, twN, nfr);
+    fft_inplace<LOGM, kThreads>(work, twN, nfr);
 
     // overlap-add; work now holds real frames: frame fr, sample n at ((float*)work)[fr*N + n]
     const float* frames = reinterpret_cast<const float*>(work);

@@ -9,12 +9,16 @@
 * ``enhance_batch(model, signals)``          -- many clips of different lengths (reference ``test.py`` / ``evaluate.py``,
   many-file ``predict.py``): sorted by length and run in ragged batches (``AeroEngine.forward_varlen``), each clip with
   the result it gets on its own.
+* ``evaluate_batch(model, lr, hr)``           -- reference ``src/evaluate.py:143-185`` ``evaluate()`` without ViSQOL, wandb and
+  file writing: every file's estimate, ``match_signal`` to its ``hr`` length, the per-file LSDs of one fused call
+  (``metrics.get_lsd_batch``) and their mean over files with a non-zero LSD, averaged over ranks.
 """
 from __future__ import annotations
 
 import math
 
 import torch
+import torch.nn.functional as F
 
 SEGMENT_DURATION_SEC = 10          # reference predict.py:22
 
@@ -94,3 +98,51 @@ def enhance_batch(model, signals, max_batch=32, return_spec=False, return_lr_spe
             else:
                 results[i] = r
     return results
+
+
+def match_signal(signal, ref_len):
+    """reference src/utils.py:211-217: crop or zero-pad the last axis of `signal` to `ref_len` samples."""
+    n = signal.shape[-1]
+    if n < ref_len:
+        return F.pad(signal, (0, ref_len - n))
+    return signal[..., :ref_len]
+
+
+def nonzero_mean(values):
+    """reference evaluate.py:160-177: the sum of the per-file values over the number of files whose value is not 0 (a file
+    scored 0 does not count); (0.0, 0) when there is none.  Returns (mean, count)."""
+    values = [float(v) for v in values]
+    count = sum(1 for v in values if v != 0)
+    return (sum(values) / count if count else 0.0), count
+
+
+@torch.no_grad()
+def evaluate_batch(model, lr_signals, hr_signals, max_batch=32):
+    """lr_signals, hr_signals: lists of [C, L_i] CUDA tensors (the model's input and the high-rate target of each file).
+    AERO runs the files through ``enhance_batch`` (ragged batches of at most ``max_batch``), SEANet file by file.  Each
+    estimate is cropped or zero-padded to its target's length and all files are scored in one ``get_lsd_batch`` call.
+    Returns (per-file LSDs as an fp32 CUDA tensor [N], the mean over files with a non-zero LSD, that count); under
+    ``torch.distributed`` the mean is averaged over ranks weighted by each rank's count.  Like the reference, the model
+    runs in eval mode and is put back in the mode it came in."""
+    from .metrics import get_lsd_batch
+    from .model import Aero
+    from .parallel import average_over_ranks
+    from .seanet import Seanet
+    lr_signals, hr_signals = list(lr_signals), list(hr_signals)
+    if len(lr_signals) != len(hr_signals):
+        raise ValueError(f"{len(lr_signals)} inputs for {len(hr_signals)} targets")
+    if not isinstance(model, (Aero, Seanet)):
+        raise NotImplementedError(f"evaluate_batch runs AERO or SEANet, got {type(model).__name__}")
+    was_training = model.training
+    model.eval()
+    try:
+        if isinstance(model, Aero):
+            prs = enhance_batch(model, lr_signals, max_batch=max_batch)
+        else:
+            prs = [model(x[None])[0] for x in lr_signals]         # enhance_batch runs AERO only
+    finally:
+        model.train(was_training)
+    prs = [match_signal(p, h.shape[-1]) for p, h in zip(prs, hr_signals)]
+    lsd = get_lsd_batch(hr_signals, prs)
+    mean, count = nonzero_mean(lsd.tolist())
+    return lsd, average_over_ranks(mean, count), count

@@ -27,6 +27,18 @@ def reduce_max(value, device=None):
     return float(t[0])
 
 
+def average_over_ranks(value, count):
+    """reference src/ddp/distrib.py:43-55 ``average([value], count)``: the mean of `value` over ranks, each weighted by its
+    `count` (a rank with count 0 adds nothing; 0.0 when every count is 0).  Every rank must call it.  Reduces in fp64, on
+    the current CUDA device under NCCL and on the CPU otherwise."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
+        return float(value)
+    device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else None
+    t = torch.tensor([float(value) * count, float(count)], dtype=torch.float64, device=device)
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    return float(t[0] / t[1]) if t[1] else 0.0
+
+
 class ShardedAero:
     """Runs `model` on this rank's shard of a global batch; optionally all-gathers the waveforms."""
 

@@ -290,6 +290,20 @@ int aero_local_attn_fwd(const float* qkvd, void* out, const aero_attn_params* p,
 int aero_lsd_fwd(const float* z_ref, const float* z_est, double* out_sum, int32_t B, int32_t bins, int32_t frames,
                  int32_t n_fft, aero_stream_t stream);
 
+/* aero_lsd_varlen_fwd: the same distance fused with its STFTs (n_fft 2048, hop 512, periodic Hann, centred, not normalised)
+ * for rows of different lengths, one value per file.
+ * ref, est      : waveforms [rows][L_max] (fp32); row r holds lengths[r] valid samples (1024 < lengths[r] <= L_max) and is
+ *                 reflect padded by 1024 at its own two ends; samples past lengths[r] are never read.
+ * row_file      : file of each row, in [0, n_files); every file has at least one row.
+ * row_frame_off : [rows + 1] first frame of each row in frame_lsd; row r has 1 + lengths[r] / 512 frames, at most max_frames.
+ * frame_lsd     : workspace [row_frame_off[rows]], the per-frame distances (fp32).
+ * out           : [n_files] fp32, the mean over all frames of all rows of each file, summed in fp64 in a fixed order.
+ * Two launches, no atomics: each file's value depends only on its own rows, bit for bit.
+ */
+int aero_lsd_varlen_fwd(const float* ref, const float* est, int32_t rows, int32_t L_max, const int32_t* lengths,
+                        const int32_t* row_file, const int32_t* row_frame_off, int32_t max_frames, int32_t n_files,
+                        float* frame_lsd, float* out, aero_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Multi-resolution STFT loss, forward value (SURVEY.md section 8f rank 2; reference src/models/stft_loss.py:11-27,30-63,96-138).
  * z_est, z_ref : planar complex spectrograms [B][bins][frames] (float2) of the estimate and the target as written by
