@@ -150,6 +150,8 @@ SYMBOLS = {
     "aero_frame_mask_fwd": (C.c_int, [vp, vp] + [i32] * 5 + [vp]),
     "aero_gather_rows_fwd": (C.c_int, [vp, vp, vp, vp, i64, i32, i32, i32, vp]),
     "aero_local_attn_varlen_fwd": (C.c_int, [vp, vp, vp, i32, C.POINTER(AttnParams), vp]),
+    "aero_seanet_input_varlen_fwd": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.POINTER(ResampleParams), vp]),
+    "aero_reflect_act_varlen_fwd": (C.c_int, [vp, vp, vp, i32, i32, i32, i64, i64, i32, i32, i32, vp]),
 }
 
 

@@ -7,8 +7,8 @@
   host round trip per chunk; here equal-length chunks go through the kernels as one batch and stay on the device.
   Results are identical to the serial loop because samples of a batch never interact.
 * ``enhance_batch(model, signals)``          -- many clips of different lengths (reference ``test.py`` / ``evaluate.py``,
-  many-file ``predict.py``): sorted by length and run in ragged batches (``AeroEngine.forward_varlen``), each clip with
-  the result it gets on its own.
+  many-file ``predict.py``): sorted by length and run in ragged batches (``AeroEngine.forward_varlen`` for AERO,
+  ``SeanetEngine.forward_varlen`` for SEANet), each clip with the result it gets on its own.
 * ``evaluate_batch(model, lr, hr)``           -- reference ``src/evaluate.py:143-185`` ``evaluate()`` without ViSQOL, wandb and
   file writing: every file's estimate, ``match_signal`` to its ``hr`` length, the per-file LSDs of one fused call
   (``metrics.get_lsd_batch``) and their mean over files with a non-zero LSD, averaged over ranks.
@@ -57,15 +57,31 @@ def enhance_long(model, lr_sig, sr, segment_sec=SEGMENT_DURATION_SEC, max_batch=
     return torch.cat(outs, dim=-1)
 
 
+def _ragged_batches(signals, cin, max_batch):
+    """Sort clips by length and pad them into batches of at most ``max_batch``: yields (input indices, lengths, [b, cin, L_max])."""
+    order = sorted(range(len(signals)), key=lambda i: signals[i].shape[-1])
+    for k in range(0, len(order), max_batch):
+        idx = order[k:k + max_batch]
+        lens = [signals[i].shape[-1] for i in idx]
+        mix = signals[idx[0]].new_zeros(len(idx), cin, max(lens))
+        for j, i in enumerate(idx):
+            mix[j, :, :lens[j]] = signals[i]
+        yield idx, lens, mix
+
+
 @torch.no_grad()
 def enhance_batch(model, signals, max_batch=32, return_spec=False, return_lr_spec=False):
     """signals: list of [C, L_i] tensors on the model's (CUDA) device at ``model.lr_sr``.  Returns a list, in input order,
     of what ``model(signals[i][None])`` returns with the batch axis dropped: the waveform [C_out, out_len(L_i)], and with
-    ``return_spec`` / ``return_lr_spec`` the spectrograms cropped to the clip's own frames.  Clips are sorted by length and
-    run in ragged batches of at most ``max_batch``, so that each batch carries as little padding as possible."""
+    ``return_spec`` / ``return_lr_spec`` (AERO only) the spectrograms cropped to the clip's own frames.  Clips are sorted by
+    length and run in ragged batches of at most ``max_batch``, so that each batch carries as little padding as possible.
+    ``model`` is an ``Aero`` or a ``Seanet`` in ``eval()`` mode (``AeroEngine.forward_varlen``, ``SeanetEngine.forward_varlen``)."""
     from .model import Aero
+    from .seanet import Seanet
+    if isinstance(model, Seanet):
+        return _enhance_batch_seanet(model, signals, max_batch, return_spec or return_lr_spec)
     if not isinstance(model, Aero):
-        raise NotImplementedError(f"enhance_batch runs the AERO generator only, got {type(model).__name__}")
+        raise NotImplementedError(f"enhance_batch runs the AERO or SEANet generator, got {type(model).__name__}")
     eng = model._engine()
     if model.training:
         eng._check_mode()
@@ -79,14 +95,8 @@ def enhance_batch(model, signals, max_batch=32, return_spec=False, return_lr_spe
         eng._require(s)
         if s.dim() != 2 or s.shape[0] != cin:
             raise ValueError(f"signal {i}: expected [{cin}, L], got {tuple(s.shape)}")
-    order = sorted(range(len(signals)), key=lambda i: signals[i].shape[-1])
     results = [None] * len(signals)
-    for k in range(0, len(order), max_batch):
-        idx = order[k:k + max_batch]
-        lens = [signals[i].shape[-1] for i in idx]
-        mix = signals[idx[0]].new_zeros(len(idx), cin, max(lens))
-        for j, i in enumerate(idx):
-            mix[j, :, :lens[j]] = signals[i]
+    for idx, lens, mix in _ragged_batches(signals, cin, max_batch):
         out = eng.forward_varlen(mix, lens, return_spec=return_spec, return_lr_spec=return_lr_spec)
         y, out_lens = out[0], out[1]
         frames = [model.geom.frames(n) for n in lens]
@@ -97,6 +107,37 @@ def enhance_batch(model, signals, max_batch=32, return_spec=False, return_lr_spe
                 results[i] = (r, *specs)
             else:
                 results[i] = r
+    return results
+
+
+def _enhance_batch_seanet(model, signals, max_batch, specs):
+    # everything a SEANet call can be refused for is checked on the host, in this order, before the engine is built or the
+    # library is loaded: the mode, the arguments, then each clip's shape and length (the error names the clip)
+    if model.training:
+        raise NotImplementedError("enhance_batch runs the SEANet inference forward; call model.eval()")
+    if specs:
+        raise ValueError("return_spec / return_lr_spec: SEANet is a time-domain generator and has no spectrogram output")
+    if max_batch < 1:
+        raise ValueError(f"max_batch must be >= 1, got {max_batch}")
+    signals = list(signals)
+    if not signals:
+        return []
+    cin = model.in_channels
+    for i, s in enumerate(signals):
+        if s.dim() != 2 or s.shape[0] != cin:
+            raise ValueError(f"signal {i}: expected [{cin}, L], got {tuple(s.shape)}")
+        try:
+            model.check_length(s.shape[-1])
+        except ValueError as e:
+            raise ValueError(f"signal {i}: {e}") from None
+    eng = model._engine()
+    for s in signals:
+        eng._require(s)
+    results = [None] * len(signals)
+    for idx, lens, mix in _ragged_batches(signals, cin, max_batch):
+        y, out_lens = eng.forward_varlen(mix, lens)
+        for j, i in enumerate(idx):
+            results[i] = y[j, :, :out_lens[j]].clone()
     return results
 
 
@@ -119,7 +160,7 @@ def nonzero_mean(values):
 @torch.no_grad()
 def evaluate_batch(model, lr_signals, hr_signals, max_batch=32):
     """lr_signals, hr_signals: lists of [C, L_i] CUDA tensors (the model's input and the high-rate target of each file).
-    AERO runs the files through ``enhance_batch`` (ragged batches of at most ``max_batch``), SEANet file by file.  Each
+    Both generators run the files through ``enhance_batch`` (ragged batches of at most ``max_batch``).  Each
     estimate is cropped or zero-padded to its target's length and all files are scored in one ``get_lsd_batch`` call.
     Returns (per-file LSDs as an fp32 CUDA tensor [N], the mean over files with a non-zero LSD, that count); under
     ``torch.distributed`` the mean is averaged over ranks weighted by each rank's count.  Like the reference, the model
@@ -136,10 +177,7 @@ def evaluate_batch(model, lr_signals, hr_signals, max_batch=32):
     was_training = model.training
     model.eval()
     try:
-        if isinstance(model, Aero):
-            prs = enhance_batch(model, lr_signals, max_batch=max_batch)
-        else:
-            prs = [model(x[None])[0] for x in lr_signals]         # enhance_batch runs AERO only
+        prs = enhance_batch(model, lr_signals, max_batch=max_batch)
     finally:
         model.train(was_training)
     prs = [match_signal(p, h.shape[-1]) for p, h in zip(prs, hr_signals)]

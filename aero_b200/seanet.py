@@ -9,6 +9,7 @@ Layout: channels-last ``[B, frames, C]``.  Every activation that feeds a reflect
 ``max dilation`` frames per clip by ``aero_reflect_act_fwd`` (LeakyReLU + reflection in one pass), so the convolution reads it
 with no padding.  Strided convolutions and transposed convolutions run on the tap-GEMM over "super-frames": ``[B, T, C]`` viewed
 as ``[B, T/r, r*C]`` (see ``superframe_conv_weight`` / ``superframe_convt_weight`` and DESIGN.md, "SEANet").
+``SeanetEngine.forward_varlen`` runs clips of different lengths in one forward, each bit-identical to its own (DESIGN.md section 14).
 """
 from __future__ import annotations
 
@@ -26,7 +27,8 @@ from .discriminator import _DiscEngine
 from .model import _record_ctor_args
 from .train_engine import TrainEngine, _Conv
 
-__all__ = ["Seanet", "SeanetEngine", "SeanetTrainEngine", "sinc_resample_table", "superframe_conv_weight", "superframe_convt_weight"]
+__all__ = ["Seanet", "SeanetEngine", "SeanetTrainEngine", "seanet_ragged_tables", "sinc_resample_table", "superframe_conv_weight",
+           "superframe_convt_weight"]
 
 _SLOPE = 0.2          # nn.LeakyReLU(0.2), seanet.py:14,58
 
@@ -74,6 +76,51 @@ def sinc_resample_table(orig_freq, new_freq, dtype=torch.float32, lowpass_filter
     kern = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
     kern *= window * (base / orig)
     return kern.view(new, -1), width, orig, new
+
+
+def seanet_ragged_tables(model, lengths):
+    """Per-clip length tables of a ragged SEANet batch, in integer arithmetic on the host (numpy, no device): for clip b of
+    lengths[b] low-rate samples, ``hr[b]`` = its high-rate length (``model.hr_length``), ``frames[i][b]`` = its frames at U-Net
+    level i (``model.level_lengths``; level 0 is its valid length, ``estimate_output_length(hr[b])``) and ``out_lens[b]`` =
+    min(target, valid length), the samples ``model(clip[None])`` returns.  Returns int32 arrays (hr [B], frames
+    [levels + 1, B], out_lens [B])."""
+    import numpy as np
+    n = np.asarray([int(v) for v in lengths], np.int64)
+    g = math.gcd(int(model.lr_sr), int(model.hr_sr))
+    up, orig = int(model.hr_sr) // g, int(model.lr_sr) // g
+    hr = (up * n + orig - 1) // orig if model.upsample else n.copy()
+    t = hr.copy()
+    for s in model.ratios[::-1]:                                  # encoder: strided conv, k = 2s, pad p = s//2 + s%2
+        p = s // 2 + s % 2
+        t = np.maximum(-((2 * s - 2 * p - t) // s) + 1, 1)        # max(ceil((t - 2s + 2p) / s) + 1, 1)
+    for s in model.ratios:                                        # decoder: transposed conv, output_padding s%2
+        p = s // 2 + s % 2
+        t = (t - 1) * s + 2 * s - 2 * p + s % 2
+    frames = [t]
+    for r in model.ratios[::-1]:
+        frames.append(frames[-1] // r)
+    target = n * model.scale_factor if model.upsample else n
+    out_lens = np.minimum(target, t)
+    return hr.astype(np.int32), np.stack(frames).astype(np.int32), out_lens.astype(np.int32)
+
+
+class _SeanetRagged:
+    """Per-call state of a ragged SEANet batch (SeanetEngine.forward_varlen): the clips' sample lengths, high-rate lengths,
+    output lengths and frames at every level as int32 device tables, uploaded from pinned memory in ONE asynchronous copy
+    (no host synchronisation in the launch sequence).  ``frames_d`` maps a level's buffer frame count (the longest clip's)
+    to that level's table."""
+
+    def __init__(self, model, lengths, L_max, device):
+        import numpy as np
+        hr, frames, out_lens = seanet_ragged_tables(model, lengths)
+        self.out_lens = [int(v) for v in out_lens]
+        parts = [np.asarray(lengths, np.int32), hr, out_lens, frames.reshape(-1)]
+        flat = torch.from_numpy(np.concatenate(parts))
+        if torch.device(device).type == "cuda":
+            flat = flat.pin_memory().to(device, non_blocking=True)
+        B = len(lengths)
+        self.lengths_d, self.hr_d, self.out_lens_d = flat[:B], flat[B:2 * B], flat[2 * B:3 * B]
+        self.frames_d = {T: flat[(3 + i) * B:(4 + i) * B] for i, T in enumerate(model.level_lengths(L_max))}
 
 
 def superframe_conv_weight(w, r):
@@ -331,11 +378,16 @@ class SeanetEngine(AeroEngine):
 
     # ------------------------------------------------------------------ kernel wrappers
     def _reflect_act(self, x, y, *, B, T, C, x_sb, y_sb, halo, act=ACT_LEAKY):
-        """y (pointing at frame 0 of a halo'd buffer) = act(x) with `halo` reflected frames on both sides."""
+        """y (pointing at frame 0 of a halo'd buffer) = act(x) with `halo` reflected frames on both sides.  In a ragged batch
+        each clip is reflected at its own end and followed by zeros (aero_reflect_act_varlen_fwd with the level's frame table)."""
         flags = (cabi.TG_A_F16 if x.dtype == torch.float16 else 0) | (cabi.TG_OUT_F16 if y.dtype == torch.float16 else 0) | \
                 (cabi.TG_ROUND_TF32 if self.precision >= 1 else 0)
-        cabi.check(self.lib.aero_reflect_act_fwd(_ptr(x), _ptr(y), B, T, C, x_sb, y_sb, halo, act, flags, self._stream()),
-                   self.lib)
+        if self._vl is not None:
+            rc = self.lib.aero_reflect_act_varlen_fwd(_ptr(x), _ptr(y), _ptr(self._vl.frames_d[T]), B, T, C, x_sb, y_sb, halo, act,
+                                                      flags, self._stream())
+        else:
+            rc = self.lib.aero_reflect_act_fwd(_ptr(x), _ptr(y), B, T, C, x_sb, y_sb, halo, act, flags, self._stream())
+        cabi.check(rc, self.lib)
 
     def _halo_buf(self, name, B, T, C):
         """[B, T + 2*halo, C] activation buffer (zero-filled once: halo frames a pass does not write stay finite)."""
@@ -366,6 +418,42 @@ class SeanetEngine(AeroEngine):
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
+    def forward_varlen(self, signal, lengths):
+        """Ragged batch: clip b is signal[b, :, :lengths[b]] (samples past it are never read) and comes out as
+        forward(signal[b:b+1, :, :lengths[b]]) gives it.  Returns the padded waveform [B, C_out, max out_len], zero past each
+        clip's own output length, and the list of those lengths.  Runs eagerly (no CUDA graph); its workspaces are released
+        when it returns."""
+        self._require(signal)
+        self._check_mode()
+        m = self.model
+        if signal.dim() != 3 or signal.shape[1] != m.in_channels:
+            raise ValueError(f"expected input [B, {m.in_channels}, L], got {tuple(signal.shape)}")
+        lengths = [int(n) for n in lengths]
+        if len(lengths) != signal.shape[0]:
+            raise ValueError(f"{len(lengths)} lengths for a batch of {signal.shape[0]}")
+        if not lengths:
+            return self._forward(signal), []
+        L = signal.shape[2]
+        for b, n in enumerate(lengths):
+            if not 1 <= n <= L:
+                raise ValueError(f"clip {b}: length {n} outside [1, {L}]")
+            try:
+                m.check_length(n)
+            except ValueError as e:
+                raise ValueError(f"clip {b} of {n} samples: {e}") from None
+        with self._on_device():
+            self._vl = _SeanetRagged(m, lengths, L, signal.device)
+            try:
+                y = self._forward(signal)
+                out_lens = self._vl.out_lens
+            finally:
+                self._vl = None
+                # keyed on the batch's exact longest clip, which rarely repeats in an evaluation loop: release, as AERO does
+                self._bufsets.pop((tuple(signal.shape), self.precision, "varlen"), None)
+                self._bufs = {}
+        return y[:, :, :max(out_lens)], out_lens
+
+    @torch.no_grad()
     def _forward(self, signal, return_spec=False, return_lr_spec=False):
         self._require(signal)
         self._check_mode()
@@ -379,7 +467,8 @@ class SeanetEngine(AeroEngine):
             return signal.new_zeros(0, m.out_channels, target)
         m.check_length(L)
         W = self._weights()
-        self._select_shape_set((tuple(signal.shape), self.precision))
+        vl = self._vl                   # _SeanetRagged while forward_varlen runs
+        self._select_shape_set((tuple(signal.shape), self.precision) + (() if vl is None else ("varlen",)))
         H = self.halo
         lev = m.level_lengths(L)
         Lv, L_hr = lev[0], m.hr_length(L)
@@ -394,8 +483,14 @@ class SeanetEngine(AeroEngine):
         else:
             filt, width, orig, up, taps = None, 0, 1, 0, 0
         p = cabi.ResampleParams(B, Cin, L, orig, up, width, taps, L_hr, Lv, H, 3, 1 if m.normalize else 0, float(m.floor))
-        cabi.check(self.lib.aero_seanet_input_fwd(_ptr(signal.contiguous()), _ptr(filt), _ptr(affine), _ptr(x0), C.byref(p),
-                                                  self._stream()), self.lib)
+        if vl is None:
+            rc = self.lib.aero_seanet_input_fwd(_ptr(signal.contiguous()), _ptr(filt), _ptr(affine), _ptr(x0), C.byref(p),
+                                                self._stream())
+        else:
+            rc = self.lib.aero_seanet_input_varlen_fwd(_ptr(signal.contiguous()), _ptr(filt), _ptr(affine), _ptr(x0),
+                                                       _ptr(vl.lengths_d), _ptr(vl.hr_d), _ptr(vl.frames_d[Lv]), C.byref(p),
+                                                       self._stream())
+        cabi.check(rc, self.lib)
         row0 = (Lv + 2 * H) * Cin
 
         # enc0: ReflectionPad1d(3), WNConv1d(k7, Cin -> ngf), Tanh   (the halo of x0 is the reflection)
@@ -447,6 +542,9 @@ class SeanetEngine(AeroEngine):
         y = self._buf("y", B, Lv, Cout)
         self._k7(d, y, W, f"dec{nlev + 1}", B, Lv, c, Cout, ACT_TANH, residual=x0[:, H:],
                  r_s=(row0, 0, Cin), samp_affine=affine, rnd=False)
+        if vl is not None:
+            # each clip's samples past its own output length (computed from the zero padding) read as zeros
+            cabi.check(self.lib.aero_frame_mask_fwd(_ptr(y), _ptr(vl.out_lens_d), B, 1, Lv, Cout, 0, self._stream()), self.lib)
         return y[:, :min(target, Lv)].permute(0, 2, 1).contiguous()
 
 

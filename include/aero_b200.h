@@ -594,6 +594,27 @@ int aero_gather_rows_fwd(const void* src, void* dst, const int32_t* idx, const f
  *   frames[clip] frames take part (keys, queries, decay, softmax); outputs of the padded frames are not written. */
 int aero_local_attn_varlen_fwd(const float* qkvd, void* out, const int32_t* frames, int32_t rows_per_clip,
                                const aero_attn_params* p, aero_stream_t stream);
+/* aero_seanet_input_varlen_fwd: aero_seanet_input_fwd where clip b holds lengths[b] valid samples in its rows of p->L_in
+ *   samples.  p describes the buffers: p->L_hr and p->L_valid are those of a clip of p->L_in samples (the longest), and x0 has
+ *   p->L_valid + 2*p->halo frames per clip.  Each clip gets what a single-clip call of its own length writes: std of its own
+ *   lengths[b] samples (same fp64 summation order), resampled to hr_lengths[b] samples (samples at or past lengths[b] are
+ *   never read), zero padded to valid_lengths[b] frames, `fill` frames reflected at both of its own ends, affine[b] = {std, 0}.
+ *   Frames u in [valid_lengths[b] + fill, p->L_valid + p->halo) are written as zeros.
+ *   Preconditions (the caller's; they cannot be checked without reading the device tables): 2 <= lengths[b] <= p->L_in,
+ *   hr_lengths[b] = the resampled length of lengths[b] samples (= lengths[b] when p->up == 0), hr_lengths[b] <= valid_lengths[b]
+ *   <= p->L_valid and p->fill < valid_lengths[b].  Out of contract, every table entry is clamped to the buffer and no sample
+ *   outside the clip's row is read (such frames are garbage, not a fault). */
+int aero_seanet_input_varlen_fwd(const float* x, const float* filt, float* affine, float* x0, const int32_t* lengths,
+                                 const int32_t* hr_lengths, const int32_t* valid_lengths, const aero_resample_params* p,
+                                 aero_stream_t stream);
+/* aero_reflect_act_varlen_fwd: aero_reflect_act_fwd where clip b has frames[b] of the T frames (T = the longest clip's).  It
+ *   writes act(x) on [0, frames[b]), the reflection at the clip's own ends on [-halo, 0) and [frames[b], frames[b] + halo), and
+ *   zeros on [frames[b] + halo, T + halo); frames[b] and past of x are never read.  With halo = 0 this is the input of a
+ *   zero-padded convolution (SEANet's strided and transposed convolutions over super-frames): the clip's frames are followed by
+ *   exact zeros.  Preconditions: halo < frames[b] <= T.  Out of contract, frames[b] is clamped to T and no frame outside
+ *   [0, T) of x is read. */
+int aero_reflect_act_varlen_fwd(const void* x, void* y, const int32_t* frames, int32_t B, int32_t T, int32_t C, int64_t x_sb,
+                                int64_t y_sb, int32_t halo, int32_t act, int32_t flags, aero_stream_t stream);
 
 #ifdef __cplusplus
 }
